@@ -1,6 +1,6 @@
-"""bench.py -- headline metric of BASELINE.json on B200: whisper-large-v3 tokens/sec (and RTF) on 30 s chunks.
+"""bench.py -- headline metric of BASELINE.json on H100: whisper-large-v3 tokens/sec (and RTF) on 30 s chunks.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one pass of the hot path over one batch of synthetic 30 s chunks on every rank:
@@ -40,12 +40,12 @@ def _peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return float(d.get("hbm_gbs", 6650.0)), "measured"
-    return 6650.0, "fallback"
+        return float(d.get("hbm_gbs", 3350.0)), "measured"
+    return 3350.0, "fallback (H100 SXM data sheet)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
 
     def __init__(self, index: int):
         self.index = index
@@ -88,24 +88,6 @@ class ClockSampler:
                 pass
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": mx, "reasons": sorted(reasons),
                 "samples": len(sm)}
-
-
-def ncu_traffic_bytes():
-    """DRAM bytes of one decoder-step kernel launch from the committed `ncu --set full` capture (profiles/*_mega_ncu_raw.csv:
-    dram__bytes_read.sum + dram__bytes_write.sum) -- a measurement taken under the profiler, reported beside the live
-    CUDA-event numbers, never instead of them.  None when no capture is committed."""
-    import csv
-    import glob
-
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "*_mega_ncu_raw.csv")))
-    if not files:
-        return None, None
-    scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9, "Tbyte": 1e12}
-    tot = 0.0
-    for row in csv.reader(open(files[-1])):
-        if len(row) == 3 and row[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-            tot += float(row[2]) * scale.get(row[1], 1.0)
-    return (tot or None), os.path.relpath(files[-1], ROOT)
 
 
 def decode_bytes_per_step(dims, S: int, A: int, t_mean: float) -> float:
@@ -181,6 +163,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (token ids, encoder output) as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -234,7 +218,7 @@ def main():
     prompt = np.array([[S.SOT, S.LANG_EN, S.TRANSCRIBE, S.NOTIMESTAMPS]] * A, dtype=np.int32)
     pcm = np.stack([S.synth_audio(CHUNK_S, seed=1000 + rank * A + i) for i in range(A)])
     pcm_dev = torch.from_numpy(pcm).to(dev)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 50 MB L2 of the H100
     gk = {"num_beams": 1, "do_sample": False, "language": "en", "task": "transcribe", "max_new_tokens": NEW_TOKENS}
 
     def step_resident():
@@ -277,6 +261,8 @@ def main():
     if rank == 0:
         sampler.start()
     ms_res = timed(step_resident, args.steps, args.warmup)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, A, prompt.shape[1])
     k0 = eng.decode_kernel_launches()
     ms_e2e = timed(step_e2e, args.steps, args.warmup)
     # decoder kernels of ONE e2e step, counted from the captured step graphs (warm-up steps included in the delta)
@@ -321,7 +307,6 @@ def main():
         return
     hbm, how = _peaks()
     bytes_step = decode_bytes_per_step(dims, eng.S, A, 4 + NEW_TOKENS / 2)
-    traffic, traffic_src = ncu_traffic_bytes() if (A == 1 and PRESET == "large-v3") else (None, None)
     achieved = bytes_step / (step_ms * 1e-3) / 1e9
     tokens = A * NEW_TOKENS * world
     # log-mel (2) + conv stem (2) + 7 per encoder layer (2 LayerNorm, 4 GEMMs, attention) + final LayerNorm + cross K/V projections (2 per decoder layer)
@@ -345,8 +330,7 @@ def main():
         "clocks": clocks,
         "roofline": {"bound": "hbm", "kernel": ("decode_mega_kernel (one persistent kernel per decoder step: 32 layers + LM head + greedy select)"
                                                  if mega else "decoder step (per-op gemv/attention/select kernels, one CUDA graph)"), "achieved": achieved,
-                     "peak": hbm, "unit": "GB/s", "frac": achieved / hbm, "peak_source": how, "traffic": traffic,
-                     "traffic_source": traffic_src,
+                     "peak": hbm, "unit": "GB/s", "frac": achieved / hbm, "peak_source": how,
                      "bytes_per_step": bytes_step, "ms_per_decoder_step": step_ms},
     }
     try:
@@ -355,11 +339,11 @@ def main():
             flop = A * (dims.enc_layers * (2.0 * S_enc * (4 * d * d + 2 * d * ffn) + 4.0 * S_enc * S_enc * d) + dims.dec_layers * 2 * 2.0 * S_enc * d * d)
             pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
             tf = flop / (enc_ms * 1e-3) / 1e12
-            line["encoder"] = {"bound": "tensor", "kernel": "encoder pass: gemm_tc2_kernel (tcgen05 CTA pairs) + attn_enc_tc2_kernel, one CUDA graph", "chunks": A,
+            line["encoder"] = {"bound": "tensor", "kernel": "encoder pass: gemm_tc2_kernel + attn_enc_kernel (wgmma), one CUDA graph", "chunks": A,
                                "ms_per_pass": enc_ms, "flop_per_pass": flop, "achieved": tf, "unit": "TFLOP/s",
                                "peak_sustained": pk.get("bf16_tflops_sustained"), "peak_burst": pk.get("bf16_tflops"),
                                "frac_sustained": tf / pk["bf16_tflops_sustained"] if pk.get("bf16_tflops_sustained") else None,
-                               "note": "informational; B = 1 is the latency-bound case (profiles/r2jn_summary.md: 0.65 of sustained at 64 chunks)"}
+                               "note": "informational; B = 1 is the latency-bound case"}
     except Exception as ex:  # informational entry: never at the cost of the line
         line["encoder"] = {"error": repr(ex)}
     line["configs"] = configs
@@ -375,6 +359,16 @@ def main():
     print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir: str, eng, A: int, plen: int) -> None:
+    """What the last timed resident step computed, as a caller of that path receives it: the generated token ids [A, NEW_TOKENS]
+    (float64, exact) and the encoder output [A, S, d_model] (float32).  The inputs are seeded, so two builds run with the same
+    arguments can be compared output for output."""
+    os.makedirs(out_dir, exist_ok=True)
+    toks, _, _ = eng.decode_read()
+    np.save(os.path.join(out_dir, "tokens.npy"), toks[:A, plen:plen + NEW_TOKENS].astype(np.float64))
+    np.save(os.path.join(out_dir, "encoder_output.npy"), eng.encoder_output(A).cpu().numpy().astype(np.float32))
 
 
 def extra_configs(model, weights, dev, rank, world, dist):
@@ -439,7 +433,7 @@ def cpu_baseline():
 
 
 def hf_cuda_leg(dev):
-    """Informational (BASELINE.md section 3): the reference's HF class with device='cuda' on the same B200, same workload, fp16 and
+    """Informational (BASELINE.md section 3): the reference's HF class with device='cuda' on the same GPU, same workload, fp16 and
     bf16 (sdpa attention), outside every timed region of the b200 arm.  Not the parity oracle and not the reference arm."""
     import torch
 

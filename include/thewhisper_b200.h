@@ -1,7 +1,7 @@
-/* thewhisper_b200 -- C-ABI of the B200-native Whisper hot path (log-mel -> encoder -> decoder -> tokens).
+/* thewhisper_b200 -- C-ABI of the H100-native Whisper hot path (log-mel -> encoder -> decoder -> tokens).
  *
  * This is the drop-in boundary below `thestage_speechkit.nvidia.ASRPipeline.__call__`
- * (reference: /root/reference/thestage_speechkit/nvidia/asr_pipeline.py:30-92).  The reference has no native
+ * (reference: thestage_speechkit/nvidia/asr_pipeline.py:30-92).  The reference has no native
  * code and no FFI: everything numeric is reached through `transformers` (un-vendored), so each entry point cites
  * the Python call it replaces (TF = transformers 5.5.0 as installed; the reference pins 4.52.3):
  *
@@ -160,7 +160,7 @@ int bw_host_decode_asr(bw_host_vocab* v, const int32_t* tokens, const int32_t* l
                        int32_t default_language, const char** json_out, int64_t* json_len);
 
 /* ---- single-op entry points (used by the parity tests; same kernels as the engine) --------------------------- */
-/* C[M,N] = epi(A[M,K] W[N,K]^T): impl 0 = tcgen05, 1 = CUDA-core comparator, 2 = tcgen05 CTA pairs (cta_group::2, persistent).  out_is_f32 selects the output type. */
+/* C[M,N] = epi(A[M,K] W[N,K]^T): impl 0 = wgmma (per-item tiles), 1 = CUDA-core comparator, 2 = wgmma over flat rows with specialised epilogues.  out_is_f32 selects the output type. */
 int bw_op_gemm(const void* A, const void* W, int32_t M, int32_t N, int32_t K, const float* bias, float alpha, int32_t act,
                const float* residual, void* out, int32_t out_is_f32, int32_t impl, int32_t force_bn, void* stream);
 /* The two building blocks of the batched (tensor-core) decoder step.  Split-K GEMM: split z of `ksplit` writes the raw fp32 partial
@@ -178,8 +178,8 @@ int bw_op_gelu_bias(const float* partials, int32_t nsplit, const float* bias, vo
 int bw_op_resid_ln(float* x, const float* partials, int32_t nsplit, const float* bias, const float* ln_g, const float* ln_b, void* y_bf16,
                    int32_t Q, int32_t D, void* stream);
 /* qkv [B*S, 3D] bf16 -> out [B*S, D] bf16; vt_scratch [B, H, 64, Spad] bf16 (Spad = S rounded up to 8).
-   impl 0 = tcgen05 (one query tile per CTA), 1 = CUDA-core comparator, 2 = tcgen05 ping-pong (two query tiles per CTA, O in TMEM),
-   3 = ping-pong reading V tiles from the qkv rows as an MN-major operand (vt_scratch unused). */
+   impl 0 (or 2, the value earlier builds gave their second kernel) = wgmma with V from the transposed copy in vt_scratch,
+   1 = CUDA-core comparator, 3 = the wgmma kernel reading V tiles from the qkv rows as an MN-major operand (vt_scratch unused). */
 int bw_op_attn_enc(const void* qkv, void* vt_scratch, void* out, int32_t B, int32_t S, int32_t H, int32_t impl, void* stream);
 int bw_op_layernorm(const float* x, const float* g, const float* b, void* out, int32_t out_is_f32, int32_t rows, int32_t D,
                     void* stream);

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE (oracle/): random inputs for the token-ids -> text / chunks post-processing, and the checker side of the
 comparison: the installed `WhisperTokenizer._decode_asr` (TF/models/whisper/tokenization_whisper.py) with the seam merge the reference
-installs over transformers' (REF thestage_speechkit/__init__.py:137-139) -- the real one when /root/reference is importable (golden
+installs over transformers' (REF thestage_speechkit/__init__.py:137-139) -- the real one when the reference is importable (golden
 minting, oracle/make_golden.py --only decode_asr), else its restatement oracle/hf_ref.lcs_merge (pinned to the real one by
 tests/golden/lcs_cases.json).  Only tests/ and oracle/make_golden.py import this file.
 

@@ -2,7 +2,7 @@
 
 CPU restatement of the reference's NVIDIA/HF hot path, i.e. what
 `thestage_speechkit.nvidia.ASRPipeline(model_size=None)` computes
-(REF = /root/reference, TF = installed transformers 5.5.0; the reference pins 4.52.3):
+(REF = a checkout of TheStageAI/TheWhisper, TF = installed transformers 5.5.0; the reference pins 4.52.3):
 
   * REF/thestage_speechkit/nvidia/asr_pipeline.py:15-27   patch_hf_model      -> interpolate_positions()
   * REF/thestage_speechkit/nvidia/asr_pipeline.py:30-92   ASRPipeline         -> RefASRPipeline
@@ -14,7 +14,7 @@ CPU restatement of the reference's NVIDIA/HF hot path, i.e. what
 The arithmetic lives in the third-party dependency `transformers` (un-vendored; present in this
 image on both the build container and the GPU box), so this module *drives* it exactly the way the
 reference does and restates only the reference's own glue.  It is pinned by
-`oracle/make_golden.py`, which imports the real reference from /root/reference in the build
+`oracle/make_golden.py`, which imports the real reference from such a checkout in the build
 container, checks this restatement against it output-for-output, and writes `tests/golden/*.npz`.
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may import

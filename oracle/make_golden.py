@@ -1,8 +1,8 @@
 """Mint golden vectors from the *real* reference (build container only).
 
-    PYTHONPATH=/root/reference:/root/repo python oracle/make_golden.py [--large]
+    THESTAGE_REFERENCE=<checkout of TheStageAI/TheWhisper> python oracle/make_golden.py [--large]
 
-Imports `thestage_speechkit` from /root/reference (it cannot travel to the GPU box), runs its own
+Imports `thestage_speechkit` from that checkout (it does not travel with the tests), runs its own
 `ASRPipeline` (HF branch) and its own `_find_longest_common_sequence` on deterministic synthetic
 inputs, asserts that the restatement in oracle/hf_ref.py reproduces them output-for-output, and writes
 small fixtures to tests/golden/.  This is what pins the oracle (task statement ③); the reference
@@ -29,7 +29,11 @@ from oracle import hf_ref  # noqa: E402
 
 def _import_reference():
     import transformers  # noqa: F401  (must be imported before the reference, SURVEY.md §8c)
-    sys.path.insert(0, "/root/reference")
+    ref = os.environ.get("THESTAGE_REFERENCE")
+    if not ref or not os.path.isdir(os.path.join(ref, "thestage_speechkit")):
+        raise SystemExit("make_golden.py: set THESTAGE_REFERENCE to a checkout of TheStageAI/TheWhisper "
+                         f"(the directory that holds thestage_speechkit/); got {ref!r}")
+    sys.path.insert(0, ref)
     import thestage_speechkit  # noqa: F401  (installs its LCS patch)
     from thestage_speechkit.nvidia import ASRPipeline
     from thestage_speechkit import _find_longest_common_sequence as ref_lcs

@@ -14,7 +14,7 @@ os.environ.setdefault("TOKENIZERS_PARALLELISM", "false")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     import warnings
 
     warnings.filterwarnings("ignore")

@@ -158,12 +158,16 @@ def test_teacher_forced_logits_and_greedy(cuda, tag, path, dtype, monkeypatch):
     eng.decode_begin(ids[None, :], 1, 1, opts)  # whole sequence is "prompt": nothing is sampled
     sigma = float(gold["tf_cols"].std())
     worst = 0.0
+    k0 = eng.decode_kernel_launches()
     for t in range(len(ids)):
         eng.decode_run(1)
         lg = eng.logits()[0].cpu().numpy()
         worst = max(worst, np.abs(lg[::997] - gold["tf_cols"][t]).max())
         top = gold["tf_top_ids"][t]
         assert np.abs(lg[top] - gold["tf_top_vals"][t]).max() < 0.08 * sigma + 1e-3
+    # the path really taken: the persistent step is <= 2 kernels (the launcher falls back silently when it declines a plan)
+    per_step = (eng.decode_kernel_launches() - k0) / len(ids)
+    assert (per_step <= 2) == (path == "mega"), (path, per_step)
     print(f"\n[{tag} {path} {dtype}] teacher-forced max |dlogit| = {worst:.5f} = {worst / sigma:.4f} sigma")
     assert worst < (0.02 if dtype == "fp16" else 0.08) * sigma + 1e-3, (worst, sigma)
     tol = 2.0 * worst

@@ -1,4 +1,4 @@
-"""Single-kernel parity (B200): each CUDA kernel, called through the C-ABI, against a plain torch fp32 reference of the
+"""Single-kernel parity: each CUDA kernel, called through the C-ABI, against a plain torch fp32 reference of the
 same op on the same inputs.  Tolerances are stated per test; operands are bf16 so the reference is computed from the
 bf16-rounded values in fp32."""
 import ctypes as C
@@ -47,6 +47,9 @@ def _ref_gemm(A, W, bias=None, alpha=1.0, act=0, residual=None):
     return y
 
 
+# Parameter ids are the suite's stable test names.  "pair*" name the flat-row launch (impl 2: gemm_tc2, one [B * rows, K] matrix,
+# epilogues specialised per use); in test_attn_enc "pingpong" is C-ABI value 2 (V from the transposed copy, as "tc") and
+# "pingpong-vdirect" value 3 (V read in place from the qkv rows).
 @pytest.mark.parametrize("impl,bn", [(1, 0), (0, 128), (0, 64), (0, 256), (0, 0), (2, 128), (2, 256), (2, 0)],
                          ids=["simt", "tc128", "tc64", "tc256", "tcauto", "pair128", "pair256", "pairauto"])
 @pytest.mark.parametrize("M,N,K", [(128, 128, 64), (256, 256, 128), (1500, 1280, 1280), (77, 384, 5120), (3000, 3840, 384),
@@ -150,7 +153,7 @@ def test_gemm_dec(cuda, Q, N, K):
 @pytest.mark.parametrize("impl,N,fbn", [(1, 640, 0), (0, 640, 0), (2, 640, 0), (2, 768, 0), (2, 640, 1128), (2, 768, 1256)],
                          ids=["simt", "tc", "pair128", "pair256", "pair128-generic", "pair256-generic"])
 def test_gemm_epilogues(cuda, impl, N, fbn):
-    """bias / alpha / GELU / fp32 residual / 16-bit or fp32 output.  The CTA-pair kernel has one specialised epilogue per combination the
+    """bias / alpha / GELU / fp32 residual / 16-bit or fp32 output.  The flat-row launch (impl 2) has one specialised epilogue per combination the
     encoder uses (GELU -> 16 bit, residual -> fp32, plain -> 16 bit) and a generic one (force_bn = 1000 + bn selects it for all)."""
     g = torch.Generator(device="cpu").manual_seed(3)
     M, K = 300, 256
@@ -182,7 +185,7 @@ def test_gemm_epilogues(cuda, impl, N, fbn):
 
 
 def test_gemm_pair_gelu_matches_erf(cuda):
-    """The CTA-pair epilogue's GELU (Abramowitz-Stegun erfc: 2 MUFU + 12 fp32 operations) against the erf GELU in float64 on a fine grid
+    """The flat-row launch's GELU (Abramowitz-Stegun erfc: 2 MUFU + 12 fp32 operations) against the erf GELU in float64 on a fine grid
     over [-9, 9]: x = hi + lo (two exact bf16 products accumulated in fp32) is steered through the accumulator, fp32 output."""
     M, N, K = 128, 16384, 64
     xs = torch.linspace(-9.0, 9.0, N)

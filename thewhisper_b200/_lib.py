@@ -1,6 +1,6 @@
 """ctypes binding of the C-ABI declared in include/thewhisper_b200.h.
 
-The shared library is built in-tree by `thewhisper_b200.build` (nvcc, sm_100a).  There is no CPU fallback: if the
+The shared library is built in-tree by `thewhisper_b200.build` (nvcc, sm_90a).  There is no CPU fallback: if the
 library is missing or no CUDA device is present, every compute call raises.
 """
 from __future__ import annotations
@@ -90,7 +90,7 @@ def load(build_if_missing: bool = False) -> C.CDLL:
 
             _build.build()
         else:
-            raise BwError(f"{LIB_PATH} not found: run `python -m thewhisper_b200.build` (nvcc, sm_100a). "
+            raise BwError(f"{LIB_PATH} not found: run `python -m thewhisper_b200.build` (nvcc, sm_90a). "
                           "thewhisper_b200 has no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SYMBOLS.items():

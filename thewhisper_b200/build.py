@@ -1,4 +1,4 @@
-"""In-tree build of the sm_100a shared library (explicit nvcc; no JIT cache, the .so travels with the repo).
+"""In-tree build of the sm_90a (H100) shared library (explicit nvcc; no JIT cache, the .so travels with the repo).
 
     python -m thewhisper_b200.build            # builds thewhisper_b200/_C/libthewhisper_b200.so if stale
 """
@@ -15,12 +15,12 @@ CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "_C")
 LIB = os.path.join(OUT_DIR, "libthewhisper_b200.so")
 # compiled twice: 16-bit elements = bfloat16 (x.o) and, with -DBW_F16, = float16 (x_f16.o)
-SOURCES_PER_DTYPE = ["api.cu", "gemm_tc.cu", "gemm_tc2.cu", "gemm_dec.cu", "attn_enc.cu", "logmel.cu", "decode.cu", "decode_stream.cu",
+SOURCES_PER_DTYPE = ["api.cu", "gemm_tc.cu", "gemm_dec.cu", "attn_enc.cu", "logmel.cu", "decode.cu", "decode_stream.cu",
                      "decode_mega.cu", "timestamps.cu"]
 SOURCES_ONCE = ["abi.cu", "hostproc.cu", "host_decode.cu"]
 HEADERS = ["common.cuh", "kernels.h", "decode.cuh", "decode_mega_common.cuh", "abi_rename.h", "abi_unrename.h",
            os.path.join("..", "..", "include", "thewhisper_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -41,7 +41,8 @@ def _stale(target: str, deps) -> bool:
 def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(OUT_DIR, exist_ok=True)
     nvcc = _nvcc()
-    hdrs = [os.path.normpath(os.path.join(CSRC, h)) for h in HEADERS]
+    # this file holds NVCC_FLAGS: objects built with other flags (another architecture) are stale too
+    hdrs = [os.path.normpath(os.path.join(CSRC, h)) for h in HEADERS] + [os.path.abspath(__file__)]
     objs, jobs = [], []
     units = [(src, "", []) for src in SOURCES_ONCE + SOURCES_PER_DTYPE] + [(src, "_f16", ["-DBW_F16"]) for src in SOURCES_PER_DTYPE]
     for src, suffix, defs in units:

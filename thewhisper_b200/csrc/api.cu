@@ -109,16 +109,15 @@ struct bw_engine {
   // batched (tensor-core) decoder step: bf16 GEMM operands [Qpad][D] / [Qpad][ffn], split-K partial sums [BSPLIT][Qm][D]
   bf16 *dbn = nullptr, *dba = nullptr, *dbh = nullptr;
   float* dpart = nullptr;
-  int batch_min = 3;  // sequences from which a step runs on the tcgen05 path (BW_BATCH_MIN)
-  bool gemm2 = true;  // encoder GEMMs on the CTA-pair kernel (BW_GEMM2=0: first-generation kernel only)
-  bool attn2 = true;  // encoder attention on the ping-pong kernel (BW_ATTN2=0: first-generation kernel)
+  int batch_min = 3;  // sequences from which a step runs on the tensor-core path (BW_BATCH_MIN)
+  bool gemm2 = true;  // encoder GEMMs on the flat-row kernel (BW_GEMM2=0: per-item kernel only)
   bool attn_vdirect = true;   // ... reading V tiles from the qkv rows (MN-major operand) instead of a transposed copy (BW_ATTN_VDIRECT=0: transposed copy)
   long long gemm2_min_rows = 1024;
   bool enc_graph = true;   // the encoder pass of a batch size runs as one CUDA graph from its second call on (BW_ENC_GRAPH=0: stream launches)
   bool enc_pdl = false;    // BW_ENC_PDL=1: ... with its kernels chained by programmatic dependent launch (measured in r2o: no gain, 5.000 vs 5.005 ms at B = 1)
   std::map<int, cudaGraphExec_t> enc_graphs;
   std::map<int, int> enc_calls;
-  int num_sms = 148;
+  int num_sms = 132;
   unsigned* mega_bar = nullptr;
   long long* mega_trace = nullptr;
   std::map<std::string, std::pair<void*, size_t>> buffers;
@@ -145,7 +144,7 @@ int need(bw_engine* e, const std::string& name, const T** out) {
 
 int gemm(bw_engine* e, cudaStream_t st, const GemmA& a, const bf16* W, int B, int rows, int N, int K, const GemmEpi& epi) {
   if (e->simt) return gemm_simt(st, a, W, B, rows, N, K, epi);
-  // plain row-major activations of all B items are one [B * rows, K] matrix: the CTA-pair kernel tiles it without per-item tails
+  // plain row-major activations of all B items are one [B * rows, K] matrix: the flat-row kernel tiles it without per-item tails
   if (e->gemm2 && a.kwrap >= K && a.pitch == K && a.batch_stride == (long long)rows * K && !epi.pos && gemm_tc2_supported(B * rows, N, K) &&
       (long long)B * rows >= e->gemm2_min_rows)
     return gemm_tc2(st, a.base, W, B * rows, N, K, rows, epi, 0);
@@ -204,11 +203,11 @@ int encode_impl(bw_engine* e, int B, cudaStream_t st) {
     if (e->simt) {
       if (int rc = attn_enc_simt(st, e->qkv, e->ao, B, S, H)) return rc;
     } else {
-      if (e->attn2 && e->attn_vdirect) {  // V tiles straight from the qkv rows (MN-major tcgen05 operand): no transposed copy
-        if (int rc = attn_enc_tc2(st, e->qkv, nullptr, e->ao, B, S, e->Spad, H)) return rc;
+      if (e->attn_vdirect) {  // V tiles straight from the qkv rows (MN-major wgmma operand): no transposed copy
+        if (int rc = attn_enc_tc(st, e->qkv, nullptr, e->ao, B, S, e->Spad, H)) return rc;
       } else {
         if (int rc = transpose_v(st, e->qkv, e->vt, B, S, e->Spad, H)) return rc;
-        if (int rc = (e->attn2 ? attn_enc_tc2 : attn_enc_tc)(st, e->qkv, e->vt, e->ao, B, S, e->Spad, H)) return rc;
+        if (int rc = attn_enc_tc(st, e->qkv, e->vt, e->ao, B, S, e->Spad, H)) return rc;
       }
     }
     {
@@ -246,12 +245,12 @@ int encode_impl(bw_engine* e, int B, cudaStream_t st) {
 
 constexpr int DPART_PER_ROW = 20480;  // floats of split-K partial sums per sequence: ksplit * N <= (SMs / n_tiles) * (n_tiles * 128) < 20480
 
-// One decoder step for Q >= 3 sequences on the tensor cores.  Every projection is a weight-streaming tcgen05 GEMM (gemm_dec.cu:
+// One decoder step for Q >= 3 sequences on the tensor cores.  Every projection is a weight-streaming wgmma GEMM (gemm_dec.cu:
 // weights = 128-row MMA operand, activations = N operand, K split so that a launch is one DRAM round trip) that leaves raw split-K
 // partial sums; the kernel that consumes them adds them in a fixed order together with bias / scale / activation:
 //   resid_ln (residual update + LayerNorm), the attention kernels (q / k / v), gelu_bias (fc1 -> fc2 operand).
 // 12 launches per layer in one CUDA graph, chained by programmatic dependent launch; weights are read once per step whatever Q is
-// (the GEMV path runs 2*Q*params flops on the fp32 pipes: 46 ms per step at Q = 64, profiles/r2a_summary.md).
+// (the GEMV path runs 2*Q*params flops on the fp32 pipes).
 int step_batched_impl(bw_engine* e, cudaStream_t st);
 int step_batched(bw_engine* e, cudaStream_t st) {
   // programmatic dependent launch for every kernel of the step (BW_PDL=0: plain stream order)
@@ -547,8 +546,6 @@ int bw_engine_create(const bw_config* cfg, bw_engine** out) {
     if (bm) e->batch_min = atoi(bm);
     const char* g2 = getenv("BW_GEMM2");
     if (g2) e->gemm2 = g2[0] != '0';
-    const char* a2 = getenv("BW_ATTN2");
-    if (a2) e->attn2 = a2[0] != '0';
     const char* eg = getenv("BW_ENC_GRAPH");
     if (eg) e->enc_graph = eg[0] != '0';
     const char* ep = getenv("BW_ENC_PDL");
@@ -568,7 +565,7 @@ int bw_engine_create(const bw_config* cfg, bw_engine** out) {
     if (fl) e->mega_flags = atoi(fl);
   }
   {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess) e->num_sms = sms;
   }
   const char* impl = getenv("BW_GEMM_IMPL");
@@ -1014,7 +1011,7 @@ int bw_op_gemm_splitk(const void* A, const void* W, int32_t M, int32_t N, int32_
 int bw_op_gemm_dec(const void* X, const void* W, int32_t Q, int32_t N, int32_t K, int32_t n_valid, int32_t want_split, float* out_partials,
                    int32_t* ksplit_used, void* stream) {
   BW_CHECK(X && W && out_partials && ksplit_used, "bw_op_gemm_dec: null pointer");
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const DecGemmPlan pl = gemm_dec_plan(Q, N, K, sms, want_split != 0);
   *ksplit_used = pl.ksplit;
@@ -1038,11 +1035,10 @@ int bw_op_attn_enc(const void* qkv, void* vt_scratch, void* out, int32_t B, int3
   BW_CHECK(qkv && out, "bw_op_attn_enc: null pointer");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (impl == 1) return attn_enc_simt(st, static_cast<const bf16*>(qkv), static_cast<bf16*>(out), B, S, H);
-  BW_CHECK(vt_scratch, "bw_op_attn_enc: vt_scratch required for the tcgen05 path");
+  BW_CHECK(vt_scratch, "bw_op_attn_enc: vt_scratch required for the tensor-core path");
   const int Spad = (S + 7) / 8 * 8;
-  if (impl == 3) return attn_enc_tc2(st, static_cast<const bf16*>(qkv), nullptr, static_cast<bf16*>(out), B, S, Spad, H);
+  if (impl == 3) return attn_enc_tc(st, static_cast<const bf16*>(qkv), nullptr, static_cast<bf16*>(out), B, S, Spad, H);
   if (int rc = transpose_v(st, static_cast<const bf16*>(qkv), static_cast<bf16*>(vt_scratch), B, S, Spad, H)) return rc;
-  if (impl == 2) return attn_enc_tc2(st, static_cast<const bf16*>(qkv), static_cast<const bf16*>(vt_scratch), static_cast<bf16*>(out), B, S, Spad, H);
   return attn_enc_tc(st, static_cast<const bf16*>(qkv), static_cast<const bf16*>(vt_scratch), static_cast<bf16*>(out), B, S, Spad, H);
 }
 

@@ -1,19 +1,16 @@
-// Encoder self-attention (non-causal, head_dim 64) as a tcgen05 flash kernel for sm_100a.
+// Encoder self-attention (non-causal, head_dim 64) as a wgmma flash kernel for sm_90a.
 //
 // Replaces SDPA / eager attention of TF/models/whisper/modeling_whisper.py:215-238,343-353 for the encoder
 // (no mask, :637-641).  softmax(q k^T * dh^-1/2) v with fp32 scores/accumulators, bf16 operands.
 //
-// One CTA = 128 query rows of one (batch, head); 192 threads:
-//   warps 0-3  softmax: one query row per thread.  S tile (128x128 fp32) is read from TMEM with tcgen05.ld,
-//              online max/sum in registers, P (bf16) written to smem in the 128B-swizzled K-major layout the
-//              PV MMA consumes; the PV partial (128x64 fp32) is read back from TMEM and folded into the
-//              running output held in registers (no TMEM read-modify-write).
-//   warp  4    TMA producer: Q once, then K / V^T tiles through a 2-deep ring (mbarrier complete_tx)
-//   warp  5    TMEM allocator + MMA issuer: S = Q K^T (4 x tcgen05.mma, N=128), O_j = P V (8 x, N=64)
-// 112 KB smem and 256 TMEM columns per CTA -> two CTAs per SM, so one CTA's exp phase overlaps the other's MMAs.
-// Keys beyond S (tile overrun into the next row block / TMA zero fill) are masked to -inf before the max.
-#include <type_traits>
-
+// One CTA = 128 query rows of one (batch, head); 288 threads:
+//   warps 0-7  two consumer warpgroups, 64 query rows each.  Per key tile of 128: S = Q K^T (4 x wgmma m64n128k16, Q and K from
+//              smem) into registers, online max / sum over the rows (a row lives in the 4 lanes of a quad), P = exp2(...) packed to
+//              bf16 in registers as the A operand of O += P V (8 x wgmma m64n64k16, A from registers); O stays in registers.
+//   warp  8    TMA producer: Q once, then K / V tiles through a KV_STAGES-deep ring (mbarrier complete_tx)
+// V is either the transposed copy vt [B, H, 64, Spad] (K-major operand) or, without a copy, the V columns of the qkv rows themselves
+// (MN-major operand: row = key, 128 B = the head's 64 dims).
+// Keys beyond S (tile overrun into the next audio's rows / TMA zero fill) are masked to -inf before the max.
 #include "kernels.h"
 
 namespace BW_NS {
@@ -25,533 +22,179 @@ constexpr int TK = 128;   // keys per tile
 constexpr int DH = 64;
 constexpr int Q_BYTES = TQ * DH * 2;       // 16 KB
 constexpr int K_BYTES = TK * DH * 2;       // 16 KB
-constexpr int V_BYTES = DH * TK * 2;       // 16 KB  (two 8 KB atoms of 64 keys)
-constexpr int P_BYTES = TQ * TK * 2;       // 32 KB  (two 16 KB atoms of 64 keys)
-constexpr int ATT_SMEM = Q_BYTES + 2 * K_BYTES + 2 * V_BYTES + P_BYTES + 128;
+constexpr int V_BYTES = DH * TK * 2;       // 16 KB  (V^T: two 8 KB atoms of 64 keys; direct: 128 rows of 128 B)
+constexpr int KV_STAGES = 3;
+constexpr int ATT_SMEM = Q_BYTES + KV_STAGES * (K_BYTES + V_BYTES) + 1024 /*align slack*/ + 256 /*barriers*/;
+constexpr int THREADS = 288;
+constexpr int CONSUMER_WARPS = 8;
 constexpr float LOG2E = 1.4426950408889634f;
 
 struct AttnParams {
   int B, S, H, D;
   float scale_log2e;  // dh^-1/2 * log2(e)
-  int v_direct = 0;   // ping-pong kernel: V tiles come straight from the qkv rows (MN-major B operand), no transposed copy
   bf16* out;
 };
 
-__global__ void __launch_bounds__(192, 2)
-attn_enc_tc_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmVT, const AttnParams p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
+template <bool VDIRECT>
+__global__ void __launch_bounds__(THREADS, 1)
+attn_enc_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmVT, const AttnParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + Q_BYTES;
-  uint8_t* sV = sK + 2 * K_BYTES;
-  uint8_t* sP = sV + 2 * V_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + P_BYTES);
-  uint64_t* q_full = bars + 0;
-  uint64_t* k_full = bars + 1;   // [2]
-  uint64_t* v_full = bars + 3;   // [2]
-  uint64_t* k_empty = bars + 5;  // [2]
-  uint64_t* v_empty = bars + 7;  // [2]
-  uint64_t* s_full = bars + 9;
-  uint64_t* p_full = bars + 10;
-  uint64_t* o_full = bars + 11;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 12);
+  uint8_t* sV = sK + KV_STAGES * K_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + KV_STAGES * V_BYTES);
+  uint64_t* q_full = bars;
+  uint64_t* kv_full = bars + 1;              // [KV_STAGES]
+  uint64_t* kv_empty = bars + 1 + KV_STAGES;  // [KV_STAGES]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * TQ, h = blockIdx.y, b = blockIdx.z;
   const int NT = (p.S + TK - 1) / TK;
 
   if (threadIdx.x == 0) {
-    if (smem_u32(smem) & 1023u) {
-      printf("[bw] attn_enc: dynamic smem base not 1024-aligned\n");
-      __trap();
-    }
     mbar_init(q_full, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&k_full[i], 1);
-      mbar_init(&v_full[i], 1);
-      mbar_init(&k_empty[i], 1);
-      mbar_init(&v_empty[i], 1);
+    for (int i = 0; i < KV_STAGES; ++i) {
+      mbar_init(&kv_full[i], 1);
+      mbar_init(&kv_empty[i], CONSUMER_WARPS);
     }
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 128);
-    mbar_init(o_full, 1);
     fence_mbar_init();
   }
-  if (warp == 4 && lane == 0) {
+  if (warp == CONSUMER_WARPS && lane == 0) {
     tma_prefetch_desc(&tmQK);
-    tma_prefetch_desc(&tmVT);
+    if (!VDIRECT) tma_prefetch_desc(&tmVT);
   }
-  if (warp == 5) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S = tmem_base;         // columns [0,128)
-  const uint32_t tmem_O = tmem_base + 128;   // columns [128,192)
+  pdl_wait();  // (programmatic dependent launch: the qkv rows are the predecessor's output)
+  pdl_launch();
 
-  if (warp == 4) {
+  if (warp == CONSUMER_WARPS) {
+    // ---------------- TMA producer ----------------
     if (lane == 0) {
       const int row0 = b * p.S;
       mbar_arrive_expect_tx(q_full, Q_BYTES);
       tma_load_2d(sQ, &tmQK, q_full, h * DH, row0 + q0);
-      for (int j = 0; j < NT; ++j) {
-        const int s = j & 1;
-        const uint32_t ph = (j >> 1) & 1;
-        mbar_wait(&k_empty[s], ph ^ 1);
-        mbar_arrive_expect_tx(&k_full[s], K_BYTES);
-        tma_load_2d(sK + s * K_BYTES, &tmQK, &k_full[s], p.D + h * DH, row0 + j * TK);
-        mbar_wait(&v_empty[s], ph ^ 1);
-        mbar_arrive_expect_tx(&v_full[s], V_BYTES);
-        const int vrow = (b * p.H + h) * DH;
-        tma_load_2d(sV + s * V_BYTES, &tmVT, &v_full[s], j * TK, vrow);
-        tma_load_2d(sV + s * V_BYTES + V_BYTES / 2, &tmVT, &v_full[s], j * TK + 64, vrow);
-      }
-    }
-  } else if (warp == 5) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16(TQ, TK);
-      constexpr uint32_t idesc_o = umma_idesc_bf16(TQ, DH);
-      const uint64_t qd = umma_desc_sw128(smem_u32(sQ));
-      mbar_wait(q_full, 0);
-      mbar_wait(&k_full[0], 0);
-      tc_fence_after();
-      {
-        const uint64_t kd = umma_desc_sw128(smem_u32(sK));
-#pragma unroll
-        for (int k = 0; k < DH / 16; ++k) umma_bf16(tmem_S, qd + 2 * k, kd + 2 * k, idesc_s, (uint32_t)(k != 0));
-        umma_commit(s_full);
-        umma_commit(&k_empty[0]);
-      }
-      for (int j = 0; j < NT; ++j) {
-        const int s = j & 1;
-        mbar_wait(p_full, j & 1);  // softmax consumed S(j) and published P(j)
-        mbar_wait(&v_full[s], (j >> 1) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < TK / 16; ++k) {
-          const uint64_t pd = umma_desc_sw128(smem_u32(sP + (k >> 2) * (P_BYTES / 2))) + 2 * (k & 3);
-          const uint64_t vd = umma_desc_sw128(smem_u32(sV + s * V_BYTES + (k >> 2) * (V_BYTES / 2))) + 2 * (k & 3);
-          umma_bf16(tmem_O, pd, vd, idesc_o, (uint32_t)(k != 0));
-        }
-        umma_commit(o_full);
-        umma_commit(&v_empty[s]);
-        if (j + 1 < NT) {
-          const int s2 = (j + 1) & 1;
-          mbar_wait(&k_full[s2], ((j + 1) >> 1) & 1);
-          tc_fence_after();
-          const uint64_t kd = umma_desc_sw128(smem_u32(sK + s2 * K_BYTES));
-#pragma unroll
-          for (int k = 0; k < DH / 16; ++k) umma_bf16(tmem_S, qd + 2 * k, kd + 2 * k, idesc_s, (uint32_t)(k != 0));
-          umma_commit(s_full);
-          umma_commit(&k_empty[s2]);
-        }
-      }
-    }
-  } else {
-    // ------------------------------ softmax / output warps ------------------------------
-    const int r = warp * 32 + lane;
-    const uint32_t lane_sel = (uint32_t)(warp * 32) << 16;
-    float m = -INFINITY, l = 0.f;
-    float o[DH];
-#pragma unroll
-    for (int i = 0; i < DH; ++i) o[i] = 0.f;
-    for (int j = 0; j < NT; ++j) {
-      mbar_wait(s_full, j & 1);
-      tc_fence_after();
-      const int key0 = j * TK;
-      // pass 1: row max over the valid keys of this tile
-      float tmax = -INFINITY;
-#pragma unroll 1
-      for (int c = 0; c < TK / 32; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_S + lane_sel + c * 32, v);
-        tmem_ld_wait();
-        const int kbase = key0 + c * 32;
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-          if (kbase + i < p.S) tmax = fmaxf(tmax, __uint_as_float(v[i]));
-      }
-      const float m_new = fmaxf(m, tmax);                     // finite: every tile has >= 1 valid key
-      const float alpha = exp2f((m - m_new) * p.scale_log2e);  // m = -inf on the first tile -> 0
-      const float mb = m_new * p.scale_log2e;
-      float lsum = 0.f;
-      // pass 2: p = exp2(s*c - m*c), bf16 P into the swizzled A-operand layout
-#pragma unroll 1
-      for (int c = 0; c < TK / 32; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_S + lane_sel + c * 32, v);
-        tmem_ld_wait();
-        const int kbase = key0 + c * 32;
-        float pf[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const float e = exp2f(fmaf(__uint_as_float(v[i]), p.scale_log2e, -mb));
-          pf[i] = (kbase + i < p.S) ? e : 0.f;
-          lsum += pf[i];
-        }
-        uint8_t* atom = sP + (c >> 1) * (P_BYTES / 2) + r * 128;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 w;
-          w.x = pack_bf16(pf[q * 8 + 0], pf[q * 8 + 1]);
-          w.y = pack_bf16(pf[q * 8 + 2], pf[q * 8 + 3]);
-          w.z = pack_bf16(pf[q * 8 + 4], pf[q * 8 + 5]);
-          w.w = pack_bf16(pf[q * 8 + 6], pf[q * 8 + 7]);
-          const int chunk = (c & 1) * 4 + q;
-          *reinterpret_cast<uint4*>(atom + ((chunk ^ (r & 7)) << 4)) = w;
-        }
-      }
-      l = l * alpha + lsum;
-      m = m_new;
-      fence_proxy_async_smem();  // P visible to the tensor core's async-proxy reads
-      tc_fence_before();         // our tcgen05.ld of S are complete before the issuer overwrites S
-      mbar_arrive(p_full);
-      // fold PV(j) into the running output
-      mbar_wait(o_full, j & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < DH / 32; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_O + lane_sel + c * 32, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[c * 32 + i] = fmaf(o[c * 32 + i], alpha, __uint_as_float(v[i]));
-      }
-    }
-    const int q = q0 + r;
-    if (q < p.S) {
-      const float inv = 1.0f / l;
-      bf16* op = p.out + ((long long)(b * p.S + q) * p.D + h * DH);
-#pragma unroll
-      for (int i = 0; i < DH; i += 8) {
-        uint4 w;
-        w.x = pack_bf16(o[i] * inv, o[i + 1] * inv);
-        w.y = pack_bf16(o[i + 2] * inv, o[i + 3] * inv);
-        w.z = pack_bf16(o[i + 4] * inv, o[i + 5] * inv);
-        w.w = pack_bf16(o[i + 6] * inv, o[i + 7] * inv);
-        *reinterpret_cast<uint4*>(op + i) = w;
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    __syncwarp();
-    tmem_dealloc(tmem_base, 256);
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------------------------------------
-// Second generation: two query tiles per CTA in ping-pong (the FlashAttention-4 schedule, restated in raw PTX).
-// Why (profiles/r2a_summary.md, r2bcd_summary.md: tensor pipe 14 %, sm__throughput 46 %): with ONE S buffer per CTA the tensor
-// pipe idles while the softmax warps exponentiate and vice versa, every key tile costs two dependent hand-overs, and the P.V
-// partial is read back from TMEM and folded into 64 registers per thread per tile.  Here
-//   * a CTA owns 256 query rows = two tiles A / B with their own S (128 TMEM columns each) and O (64 columns each) and their own
-//     softmax warpgroup (4 warps each): while group A exponentiates S_A(j), the tensor pipe runs QK_B(j) / PV_B(j-1), and K / V tiles
-//     are fetched once for 256 queries instead of once for 128;
-//   * O accumulates IN TMEM across key tiles (tcgen05.mma accumulate); a row's reference maximum is only raised when the tile maximum
-//     exceeds it by more than 2^8 (lazy rescaling: p <= 256 is harmless in bf16 / fp32), and then O is rescaled in place
-//     (tcgen05.ld -> multiply -> tcgen05.st); after the first tiles this almost never happens, so the per-tile O read-back is gone;
-//   * a softmax thread owns one query row: it pulls the 128 scores of a key tile into registers at once and hands S_g's TMEM columns straight
-//     back (s_free), so QK_g(j+1) runs under the exponentials of tile j; pv_done orders "PV_g(j) has read P_g / updated O_g" before the
-//     group rewrites P_g or rescales O_g.
-// One CTA per SM: 192 KB smem (Q 2 x 16, K ring 3 x 16, V ring 3 x 16, P 2 x 32) and 384 of the 512 TMEM columns.
-// The exp unit bounds it: 16 MUFU.EX2 / clk / SM = 2048 clk per (256 queries x 128 keys) against 1024 clk of MMAs.
-// ------------------------------------------------------------------------------------------------------------------------------
-constexpr int KV_STAGES = 3;
-constexpr int ATT2_SMEM = 2 * Q_BYTES + KV_STAGES * (K_BYTES + V_BYTES) + 2 * P_BYTES + 256;
-constexpr float LAZY_TAU = 8.0f;  // log2 units: rescale O only when the tile maximum exceeds the reference by more than this
-
-__global__ void __launch_bounds__(384, 1)
-attn_enc_tc2_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmVT, const AttnParams p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sQ = smem;                                   // [2][16 KB]
-  uint8_t* sK = sQ + 2 * Q_BYTES;                       // [KV_STAGES][16 KB]
-  uint8_t* sV = sK + KV_STAGES * K_BYTES;               // [KV_STAGES][16 KB]
-  uint8_t* sP = sV + KV_STAGES * V_BYTES;               // [2][32 KB]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * P_BYTES);
-  uint64_t* q_full = bars + 0;                 // [2]
-  uint64_t* k_full = bars + 2;                 // [KV_STAGES]
-  uint64_t* v_full = bars + 2 + KV_STAGES;     // [KV_STAGES]
-  uint64_t* k_empty = bars + 2 + 2 * KV_STAGES;
-  uint64_t* v_empty = bars + 2 + 3 * KV_STAGES;
-  uint64_t* s_full = bars + 2 + 4 * KV_STAGES;      // [2]
-  uint64_t* p_full = s_full + 2;                    // [2]
-  uint64_t* s_free = p_full + 2;                    // [2]  softmax g holds S_g(j) in registers: QK_g(j+1) may overwrite the TMEM copy
-  uint64_t* pv_done = s_free + 2;                   // [2]  PV_g(j) complete: P_g may be rewritten, O_g may be rescaled / read
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_done + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * 2 * TQ, h = blockIdx.y, b = blockIdx.z;
-  const int NT = (p.S + TK - 1) / TK;
-
-  if (threadIdx.x == 0) {
-    if (smem_u32(smem) & 1023u) {
-      printf("[bw] attn_enc2: dynamic smem base not 1024-aligned\n");
-      __trap();
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&q_full[i], 1);
-      mbar_init(&s_full[i], 1);
-      mbar_init(&p_full[i], 128);
-      mbar_init(&s_free[i], 128);
-      mbar_init(&pv_done[i], 1);
-    }
-    for (int i = 0; i < KV_STAGES; ++i) {
-      mbar_init(&k_full[i], 1);
-      mbar_init(&v_full[i], 1);
-      mbar_init(&k_empty[i], 1);
-      mbar_init(&v_empty[i], 1);
-    }
-    fence_mbar_init();
-  }
-  if (warp == 8 && lane == 0) {
-    tma_prefetch_desc(&tmQK);
-    tma_prefetch_desc(&tmVT);
-  }
-  if (warp == 9) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // columns: S_A [0,128) S_B [128,256) O_A [256,320) O_B [320,384)
-  pdl_wait();  // (programmatic dependent launch: the qkv rows are the predecessor's output)
-  pdl_launch();
-
-  // 384 threads = three warpgroups: two softmax groups and one of {TMA warp, MMA warp, two idle warps}.  A softmax thread keeps a whole
-  // 128-score row in registers, so the third group gives registers back (168 -> 56) and the softmax groups take them (168 -> 224).
-  if (warp >= 8) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-    if (warp == 8) {
-    // ---------------- TMA producer ----------------
-    if (lane == 0) {
-      const int row0 = b * p.S;
-      for (int g = 0; g < 2; ++g) {
-        mbar_arrive_expect_tx(&q_full[g], Q_BYTES);
-        tma_load_2d(sQ + g * Q_BYTES, &tmQK, &q_full[g], h * DH, row0 + q0 + g * TQ);
-      }
       const int vrow = (b * p.H + h) * DH;
       for (int j = 0; j < NT; ++j) {
         const int s = j % KV_STAGES;
-        const uint32_t ph = (j / KV_STAGES) & 1;
-        mbar_wait(&k_empty[s], ph ^ 1);
-        mbar_arrive_expect_tx(&k_full[s], K_BYTES);
-        tma_load_2d(sK + s * K_BYTES, &tmQK, &k_full[s], p.D + h * DH, row0 + j * TK);
-        mbar_wait(&v_empty[s], ph ^ 1);
-        mbar_arrive_expect_tx(&v_full[s], V_BYTES);
-        if (p.v_direct) {
-          // 128 keys x 64 dims exactly as they lie in the qkv rows: row = key, 128 B = the head's 64 dims, 128B-swizzled -- the canonical
-          // MN-major operand layout (N = 64 contiguous, 8-key groups 1024 B apart).  Keys beyond this audio are the next audio's rows (finite;
-          // their P is 0) or beyond the tensor (TMA zero fill).
-          tma_load_2d(sV + s * V_BYTES, &tmQK, &v_full[s], 2 * p.D + h * DH, row0 + j * TK);
+        mbar_wait_wg(&kv_empty[s], ((j / KV_STAGES) & 1) ^ 1);
+        mbar_arrive_expect_tx(&kv_full[s], K_BYTES + V_BYTES);
+        tma_load_2d(sK + s * K_BYTES, &tmQK, &kv_full[s], p.D + h * DH, row0 + j * TK);
+        if (VDIRECT) {
+          tma_load_2d(sV + s * V_BYTES, &tmQK, &kv_full[s], 2 * p.D + h * DH, row0 + j * TK);
         } else {
-          tma_load_2d(sV + s * V_BYTES, &tmVT, &v_full[s], j * TK, vrow);
-          tma_load_2d(sV + s * V_BYTES + V_BYTES / 2, &tmVT, &v_full[s], j * TK + 64, vrow);
+          tma_load_2d(sV + s * V_BYTES, &tmVT, &kv_full[s], j * TK, vrow);
+          tma_load_2d(sV + s * V_BYTES + V_BYTES / 2, &tmVT, &kv_full[s], j * TK + 64, vrow);
         }
       }
     }
-    } else if (warp == 9) {
-    // ---------------- MMA issuer ----------------
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16(TQ, TK);
-      constexpr uint32_t idesc_o = umma_idesc_bf16(TQ, DH);
-      auto issue_qk = [&](int g, int stage) {
-        const uint64_t qd = umma_desc_sw128(smem_u32(sQ + g * Q_BYTES));
-        const uint64_t kd = umma_desc_sw128(smem_u32(sK + stage * K_BYTES));
+    return;
+  }
+
+  // ---------------- consumer warpgroup g: query rows [q0 + 64 g, +64); this thread: rows r and r + 8 ----------------
+  const int g = warp >> 2;
+  const int r = g * 64 + (warp & 3) * 16 + (lane >> 2);
+  const uint64_t qd = wg_desc_sw128(smem_u32(sQ + g * (Q_BYTES / 2)));
+  float o[DH / 2];
 #pragma unroll
-        for (int k = 0; k < DH / 16; ++k) umma_bf16(tmem_base + g * TK, qd + 2 * k, kd + 2 * k, idesc_s, (uint32_t)(k != 0));
-      };
-      const bool v_direct = p.v_direct != 0;
-      const uint32_t idesc_pv = v_direct ? (idesc_o | (1u << 16)) : idesc_o;  // bit 16: B operand MN-major
-      auto issue_pv = [&](int g, int stage, bool acc) {
+  for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};  // m in raw score units; l: this thread's share of the row sum
+  mbar_wait_wg(q_full, 0);
+  for (int j = 0; j < NT; ++j) {
+    const int s = j % KV_STAGES;
+    mbar_wait_wg(&kv_full[s], (j / KV_STAGES) & 1);
+    float sc[TK / 2];
 #pragma unroll
-        for (int k = 0; k < TK / 16; ++k) {
-          const uint64_t pd = umma_desc_sw128(smem_u32(sP + g * P_BYTES + (k >> 2) * (P_BYTES / 2))) + 2 * (k & 3);
-          // K-major V^T: two 64-key atoms, 32 B per 16 keys inside one; MN-major V: 16 keys = 16 rows of 128 B
-          const uint64_t vd = v_direct ? umma_desc_sw128(smem_u32(sV + stage * V_BYTES + k * 2048))
-                                       : umma_desc_sw128(smem_u32(sV + stage * V_BYTES + (k >> 2) * (V_BYTES / 2))) + 2 * (k & 3);
-          umma_bf16(tmem_base + 256 + g * DH, pd, vd, idesc_pv, (uint32_t)(acc || k != 0));
-        }
-      };
-      mbar_wait(&k_full[0], 0);
-      for (int g = 0; g < 2; ++g) {
-        mbar_wait(&q_full[g], 0);
-        tc_fence_after();
-        issue_qk(g, 0);
-        umma_commit(&s_full[g]);
-      }
-      umma_commit(&k_empty[0]);  // K(0) is free once both QK(0) are done
-      // Event-driven issue: each softmax group g has at most one QK (S_g's columns handed back: s_free) and one PV (P_g published: p_full)
-      // outstanding; the issuer polls both groups and issues whatever is ready, PV first (it is what the group waits for next: pv_done
-      // guards its P buffer and O).  A fixed order (QK_A, QK_B, PV_A, PV_B) made PV_A(j) wait for group B's progress whenever the groups
-      // drift apart: 11 % of the softmax warps' time in r2j's ncu source view was that pv_done wait.
-      // QK_g(j) only needs S_g's TMEM columns back -- the group holds S_g(j-1) in registers a few hundred clocks after s_full -- so the
-      // next scores are ready long before the group has finished exponentiating.
-      int qk_j[2] = {1, 1}, pv_j[2] = {0, 0};  // next key tile per group (QK(0) was issued above)
-      int k_ready = 1, v_ready = 0;            // K / V tiles known to have landed
-      const long long t0 = clock64();
-      while (pv_j[0] < NT || pv_j[1] < NT) {
+    for (int i = 0; i < TK / 2; ++i) sc[i] = 0.f;
+    wg_fence();
+    {
+      const uint64_t kd = wg_desc_sw128(smem_u32(sK + s * K_BYTES));
 #pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          {
-            const int j = pv_j[g], s = j % KV_STAGES;
-            if (j < NT && mbar_test(&p_full[g], j & 1)) {
-              if (j >= v_ready && mbar_test(&v_full[s], (j / KV_STAGES) & 1)) v_ready = j + 1;
-              if (j < v_ready) {
-                tc_fence_after();
-                issue_pv(g, s, j > 0);
-                umma_commit(&pv_done[g]);
-                pv_j[g] = j + 1;
-                if (pv_j[g ^ 1] > j) umma_commit(&v_empty[s]);  // both groups' PV(j) are issued: V(j)'s stage is free when they complete
-              }
-            }
-          }
-          {
-            const int j = qk_j[g], s = j % KV_STAGES;
-            if (j < NT && mbar_test(&s_free[g], (j - 1) & 1)) {
-              if (j >= k_ready && mbar_test(&k_full[s], (j / KV_STAGES) & 1)) k_ready = j + 1;
-              if (j < k_ready) {
-                tc_fence_after();
-                issue_qk(g, s);
-                umma_commit(&s_full[g]);
-                qk_j[g] = j + 1;
-                if (qk_j[g ^ 1] > j) umma_commit(&k_empty[s]);
-              }
-            }
-          }
-        }
-        if (clock64() - t0 > (1ll << 32)) {  // a protocol bug must trap, not hang the box (see mbar_wait)
-          printf("[bw] attn_enc2 issuer timed out: block (%d,%d,%d) qk %d %d pv %d %d\n", blockIdx.x, blockIdx.y, blockIdx.z, qk_j[0], qk_j[1], pv_j[0],
-                 pv_j[1]);
-          __trap();
-        }
-      }
+      for (int k = 0; k < DH / 16; ++k) Wgmma<TK>::template ss<0>(sc, qd + 2 * k, kd + 2 * k, 1u);
     }
-    }  // (warps 10, 11 idle: only there so that warps 8..11 form a warpgroup for setmaxnreg)
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-    // ---------------- softmax warpgroups: g = 0 (warps 0-3) rows [q0, q0+128), g = 1 (warps 4-7) rows [q0+128, q0+256) ----------------
-    const int g = warp >> 2, wq = warp & 3;
-    const int r = wq * 32 + lane;                       // row inside the tile = TMEM lane
-    const uint32_t lane_sel = (uint32_t)(wq * 32) << 16;
-    const uint32_t tS = tmem_base + lane_sel + g * TK;
-    const uint32_t tO = tmem_base + lane_sel + 256 + g * DH;
-    uint8_t* sPg = sP + g * P_BYTES;
-    float m_ref = -INFINITY, l = 0.f;  // m_ref in raw score units
-    for (int j = 0; j < NT; ++j) {
-      mbar_wait(&s_full[g], j & 1);   // S_g(j) is complete
-      tc_fence_after();
-      const int key0 = j * TK;
-      const bool ragged = key0 + TK > p.S;  // only the last key tile has keys beyond S: the mask costs 2 of ~6 instructions per score
-      // The whole 128-score row of this thread goes to registers in one go and the TMEM copy is handed back at once (FlashAttention-4's
-      // one-thread-one-row softmax): maximum, exponentials and the bf16 pack then run from registers while the tensor pipe already
-      // computes S_g(j+1) into the same columns.
-      uint32_t sv[TK];
+    wg_commit();
+    wg_wait<0>();
+    wg_pin(sc);
+    const int key0 = j * TK;
+    if (key0 + TK > p.S) {  // only the last key tile has keys beyond S
 #pragma unroll
-      for (int c = 0; c < TK / 32; ++c) tmem_ld_32x32(tS + c * 32, *reinterpret_cast<uint32_t(*)[32]>(&sv[c * 32]));
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(&s_free[g]);
-      float tmax;
-      {
-        float t0 = -INFINITY, t1 = -INFINITY, t2 = -INFINITY, t3 = -INFINITY;
-        if (!ragged) {
+      for (int jj = 0; jj < TK / 8; ++jj)
 #pragma unroll
-          for (int i = 0; i < TK; i += 4) {
-            t0 = fmaxf(t0, __uint_as_float(sv[i]));
-            t1 = fmaxf(t1, __uint_as_float(sv[i + 1]));
-            t2 = fmaxf(t2, __uint_as_float(sv[i + 2]));
-            t3 = fmaxf(t3, __uint_as_float(sv[i + 3]));
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < TK; ++i)
-            if (key0 + i < p.S) t0 = fmaxf(t0, __uint_as_float(sv[i]));
-        }
-        tmax = fmaxf(fmaxf(t0, t1), fmaxf(t2, t3));
-      }
-      // lazy reference maximum: raise it only on the first tile or when this tile exceeds it by more than LAZY_TAU (log2 units)
-      float factor = 1.0f;
-      const bool raise = (j == 0) || ((tmax - m_ref) * p.scale_log2e > LAZY_TAU);
-      if (raise) {
-        factor = (j == 0) ? 0.f : ex2_approx((m_ref - tmax) * p.scale_log2e);
-        m_ref = tmax;
-      }
-      if (j > 0) {
-        mbar_wait(&pv_done[g], (j - 1) & 1);  // PV_g(j-1) has read P_g and updated O_g
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, raise)) {  // rescale this warp's 32 rows of O_g in place
-#pragma unroll
-          for (int c = 0; c < DH / 32; ++c) {
-            uint32_t v[32];
-            tmem_ld_32x32(tO + c * 32, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * factor);
-            tmem_st_32x32(tO + c * 32, v);
-          }
-          tmem_st_wait();
-          l *= factor;
-        }
-      }
-      const float mb = m_ref * p.scale_log2e;
-      float l0 = 0.f, l1 = 0.f, l2 = 0.f, l3 = 0.f;
-      auto exp_pack = [&](auto masked) {
-#pragma unroll
-        for (int q = 0; q < TK / 8; ++q) {  // 8 scores -> one 16-byte chunk of the swizzled P row
-          float pf[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            pf[i] = ex2_approx(fmaf(__uint_as_float(sv[q * 8 + i]), p.scale_log2e, -mb));
-            if (decltype(masked)::value && key0 + q * 8 + i >= p.S) pf[i] = 0.f;
-          }
-          l0 += pf[0] + pf[4]; l1 += pf[1] + pf[5]; l2 += pf[2] + pf[6]; l3 += pf[3] + pf[7];
-          uint4 w;
-          w.x = pack_bf16(pf[0], pf[1]);
-          w.y = pack_bf16(pf[2], pf[3]);
-          w.z = pack_bf16(pf[4], pf[5]);
-          w.w = pack_bf16(pf[6], pf[7]);
-          uint8_t* atom = sPg + (q >> 3) * (P_BYTES / 2) + r * 128;
-          *reinterpret_cast<uint4*>(atom + (((q & 7) ^ (r & 7)) << 4)) = w;
-        }
-      };
-      if (!ragged) exp_pack(std::false_type{});
-      else exp_pack(std::true_type{});
-      l += (l0 + l1) + (l2 + l3);
-      fence_proxy_async_smem();  // P visible to the tensor core's async-proxy reads
-      tc_fence_before();         // our tcgen05.st of O are complete before the issuer accumulates into it
-      mbar_arrive(&p_full[g]);
+        for (int c = 0; c < 2; ++c)
+          if (key0 + 8 * jj + 2 * (lane & 3) + c >= p.S) sc[4 * jj + c] = sc[4 * jj + 2 + c] = -INFINITY;
     }
-    // ---- final O_g
-    mbar_wait(&pv_done[g], (NT - 1) & 1);
-    tc_fence_after();
-    const int q = q0 + g * TQ + r;
-    const float inv = 1.0f / l;
-    bf16* op = p.out + ((long long)(b * p.S + q) * p.D + h * DH);
+    float alpha[2], mb[2];
 #pragma unroll
-    for (int c = 0; c < DH / 32; ++c) {
-      uint32_t v[32];
-      tmem_ld_32x32(tO + c * 32, v);
-      tmem_ld_wait();
-      if (q < p.S) {
+    for (int hh = 0; hh < 2; ++hh) {
+      float t = -INFINITY;
 #pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          uint4 w;
-          w.x = pack_bf16(__uint_as_float(v[i]) * inv, __uint_as_float(v[i + 1]) * inv);
-          w.y = pack_bf16(__uint_as_float(v[i + 2]) * inv, __uint_as_float(v[i + 3]) * inv);
-          w.z = pack_bf16(__uint_as_float(v[i + 4]) * inv, __uint_as_float(v[i + 5]) * inv);
-          w.w = pack_bf16(__uint_as_float(v[i + 6]) * inv, __uint_as_float(v[i + 7]) * inv);
-          *reinterpret_cast<uint4*>(op + c * 32 + i) = w;
-        }
+      for (int jj = 0; jj < TK / 8; ++jj) t = fmaxf(t, fmaxf(sc[4 * jj + 2 * hh], sc[4 * jj + 2 * hh + 1]));
+      t = fmaxf(t, __shfl_xor_sync(0xffffffffu, t, 1));
+      t = fmaxf(t, __shfl_xor_sync(0xffffffffu, t, 2));
+      const float m_new = fmaxf(m[hh], t);                         // finite: every tile has >= 1 valid key
+      alpha[hh] = ex2_approx((m[hh] - m_new) * p.scale_log2e);     // m = -inf on the first tile -> 0
+      mb[hh] = m_new * p.scale_log2e;
+      m[hh] = m_new;
+    }
+    // P = exp2(s c - m c) as the bf16 A fragments of the PV MMA: k-step kk covers keys [16 kk, 16 kk + 16) = chunks 2 kk, 2 kk + 1
+    uint32_t pa[TK / 16][4];
+    float ls[2] = {0.f, 0.f};
+#pragma unroll
+    for (int kk = 0; kk < TK / 16; ++kk) {
+      float pf[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        pf[i] = ex2_approx(fmaf(sc[8 * kk + i], p.scale_log2e, -mb[(i >> 1) & 1]));
+        ls[(i >> 1) & 1] += pf[i];
       }
+      pa[kk][0] = pack_bf16(pf[0], pf[1]);
+      pa[kk][1] = pack_bf16(pf[2], pf[3]);
+      pa[kk][2] = pack_bf16(pf[4], pf[5]);
+      pa[kk][3] = pack_bf16(pf[6], pf[7]);
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) l[hh] = l[hh] * alpha[hh] + ls[hh];
+#pragma unroll
+    for (int i = 0; i < DH / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+    wg_fence();
+#pragma unroll
+    for (int kk = 0; kk < TK / 16; ++kk) {
+      // MN-major V: 16 keys = 16 rows of 128 B;  K-major V^T: two 64-key atoms, 32 B per 16 keys inside one
+      const uint64_t vd = VDIRECT ? wg_desc_sw128(smem_u32(sV + s * V_BYTES + kk * 2048))
+                                  : wg_desc_sw128(smem_u32(sV + s * V_BYTES + (kk >> 2) * (V_BYTES / 2))) + 2 * (kk & 3);
+      Wgmma<DH>::template rs<VDIRECT ? 1 : 0>(o, pa[kk], vd, 1u);
+    }
+    wg_commit();
+    wg_wait<0>();
+    wg_pin(o);
+    if (lane == 0) mbar_arrive(&kv_empty[s]);  // this warp's reads of K(j) / V(j) are complete
+  }
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    float t = l[hh];
+    t += __shfl_xor_sync(0xffffffffu, t, 1);
+    t += __shfl_xor_sync(0xffffffffu, t, 2);
+    const float inv = 1.0f / t;
+    const int q = q0 + r + 8 * hh;
+    if (q < p.S) {
+      bf16* op = p.out + ((long long)(b * p.S + q) * p.D + h * DH);
+#pragma unroll
+      for (int jj = 0; jj < DH / 8; ++jj)
+        *reinterpret_cast<uint32_t*>(op + 8 * jj + 2 * (lane & 3)) = pack_bf16(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) {
-    __syncwarp();
-    tmem_dealloc(tmem_base, 512);
+}
+
+template <bool VDIRECT>
+int launch_attn(cudaStream_t st, const CUtensorMap& tmQK, const CUtensorMap& tmVT, const AttnParams& p) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    BW_CUDA_OK(cudaFuncSetAttribute(attn_enc_kernel<VDIRECT>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
+    attr_set = true;
   }
+  dim3 grid((p.S + TQ - 1) / TQ, p.H, p.B);
+  BW_CUDA_OK(launch_k(attn_enc_kernel<VDIRECT>, grid, dim3(THREADS), (size_t)ATT_SMEM, st, tmQK, tmVT, p));
+  return 0;
 }
 
 // CUDA-core sibling: one block per (query, head, batch); scores staged in smem.  Comparator / bring-up only.
@@ -613,30 +256,9 @@ __global__ void transpose_v_kernel(const bf16* __restrict__ qkv, bf16* __restric
 
 }  // namespace
 
+// vt == nullptr: no transposed copy of V, the kernel reads V tiles from the qkv rows as an MN-major operand
 int attn_enc_tc(cudaStream_t st, const bf16* qkv, const bf16* vt, bf16* out, int B, int S, int Spad, int H) {
   const int D = H * DH;
-  BW_CHECK(Spad % 8 == 0 && Spad >= S, "attn_enc: Spad=%d must be >= S and a multiple of 8", Spad);
-  CUtensorMap tmQK, tmVT;
-  if (int rc = make_tmap_2d_bf16(&tmQK, qkv, (uint64_t)B * S, (uint64_t)3 * D, (uint64_t)3 * D * 2, TQ, DH)) return rc;
-  if (int rc = make_tmap_2d_bf16(&tmVT, vt, (uint64_t)B * H * DH, (uint64_t)Spad, (uint64_t)Spad * 2, DH, 64)) return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    BW_CUDA_OK(cudaFuncSetAttribute(attn_enc_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
-    attr_set = true;
-  }
-  AttnParams p;
-  p.B = B; p.S = S; p.H = H; p.D = D;
-  p.scale_log2e = 0.125f * LOG2E;
-  p.out = out;
-  dim3 grid((S + TQ - 1) / TQ, H, B);
-  attn_enc_tc_kernel<<<grid, 192, ATT_SMEM, st>>>(tmQK, tmVT, p);
-  BW_CUDA_OK(cudaGetLastError());
-  return 0;
-}
-
-int attn_enc_tc2(cudaStream_t st, const bf16* qkv, const bf16* vt, bf16* out, int B, int S, int Spad, int H) {
-  const int D = H * DH;
-  // vt == nullptr: no transposed copy of V, the kernel reads V tiles from the qkv rows as an MN-major operand
   BW_CHECK(vt == nullptr || (Spad % 8 == 0 && Spad >= S), "attn_enc: Spad=%d must be >= S and a multiple of 8", Spad);
   CUtensorMap tmQK, tmVT;
   if (int rc = make_tmap_2d_bf16(&tmQK, qkv, (uint64_t)B * S, (uint64_t)3 * D, (uint64_t)3 * D * 2, TQ, DH)) return rc;
@@ -645,19 +267,11 @@ int attn_enc_tc2(cudaStream_t st, const bf16* qkv, const bf16* vt, bf16* out, in
   } else {
     tmVT = tmQK;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    BW_CUDA_OK(cudaFuncSetAttribute(attn_enc_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT2_SMEM));
-    attr_set = true;
-  }
   AttnParams p;
   p.B = B; p.S = S; p.H = H; p.D = D;
   p.scale_log2e = 0.125f * LOG2E;
   p.out = out;
-  p.v_direct = vt == nullptr;
-  dim3 grid((S + 2 * TQ - 1) / (2 * TQ), H, B);
-  BW_CUDA_OK(launch_k(attn_enc_tc2_kernel, grid, dim3(384), (size_t)ATT2_SMEM, st, tmQK, tmVT, p));
-  return 0;
+  return vt ? launch_attn<false>(st, tmQK, tmVT, p) : launch_attn<true>(st, tmQK, tmVT, p);
 }
 
 int attn_enc_simt(cudaStream_t st, const bf16* qkv, bf16* out, int B, int S, int H) {

@@ -1,5 +1,5 @@
-// Decoder-step kernels for sm_100a (q_len = 1): every one is a stream over weights or KV in HBM, so they are
-// plain coalesced 16-byte-load kernels sized to cover all 148 SMs; no tensor cores (SURVEY.md §8d: the step is
+// Decoder-step kernels for sm_90a (q_len = 1): every one is a stream over weights or KV in HBM, so they are
+// plain coalesced 16-byte-load kernels sized to cover all SMs; no tensor cores (SURVEY.md §8d: the step is
 // HBM-bound, 1.60 GB of weights + 245.76 MB cross-KV per audio per token).
 //
 // Replaces, per generated token, TF/models/whisper/modeling_whisper.py:449-506 (decoder layer), :738-763

@@ -32,7 +32,7 @@ struct SelfAttnArgs {
   const bf16* vc = nullptr;
   const int* anc = nullptr;    // [Q, Tmax] sequence slot holding position s for sequence q (null = own slot)
   float* out = nullptr;        // [Q, D] fp32 (per-op GEMV path) ...
-  bf16* out_bf16 = nullptr;    // ... or bf16 (operand of the batched path's tcgen05 out-projection); exactly one of the two
+  bf16* out_bf16 = nullptr;    // ... or bf16 (operand of the batched path's wgmma out-projection); exactly one of the two
   const int* pos = nullptr;
   int H = 0, D = 0, Tmax = 0;
   // batched path: the fused QKV GEMM leaves k / v of the current token in qkv (fp32, + bias); the (sequence, head) CTA rounds them to
@@ -111,7 +111,7 @@ struct MegaArgs {
   // so no phase spends registers or a dependent global load on it
   MegaLayer layers[MEGA_MAXL];
   int L, D, H, ffn, V, S, Tmax, Q;
-  int ldl;  // row pitch of logits (V rounded up to 32: rows stay 16-byte aligned for the batched path's tcgen05 LM head)
+  int ldl;  // row pitch of logits (V rounded up to 32: rows stay 16-byte aligned for the batched path's wgmma LM head)
   const bf16* embed;
   const float* dec_pos;
   const float *lnf_g, *lnf_b;

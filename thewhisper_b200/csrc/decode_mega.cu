@@ -1,12 +1,11 @@
 // One persistent kernel per decoder step (q_len = 1, one beam per audio, up to 2 sequences).
 //
 // Why: with one kernel per op the step is 259 launches and every op pays its own chain of dependent global round
-// trips; a step that should take 0.28 ms (1.86 GB at the measured 6.5 TB/s) took 1.7 ms
-// (profiles/r1_v1_launches_summary.md).  Here the whole step -- embedding, 32 x (LN1+QKV, self-attention, out-proj,
+// trips, several times the time its bytes take at HBM bandwidth.  Here the whole step -- embedding, 32 x (LN1+QKV, self-attention, out-proj,
 // LN2+cross-q, cross-attention, out-proj, LN3+fc1+GELU, fc2), final LN + tied LM head -- runs in ONE kernel of one CTA
 // per SM, phases separated by a grid barrier.
 //
-// What the barrier timelines and ncu captures of the earlier versions taught (profiles/r1_mega_timeline.md):
+// What the barrier timelines and ncu captures of the earlier versions taught:
 //   * a phase is only as fast as its chain of *dependent* L2/DRAM round trips (~0.6-1 us each), not its bytes: everything
 //     that does not depend on the previous phase is requested BEFORE the barrier that precedes a phase -- the weight rows
 //     of the phase (TMA bulk copies into a per-warp smem slab, one instruction per row: issuing the same bytes as 16-byte
@@ -34,10 +33,10 @@ using namespace mega;
 
 
 // Template parameter VAR: bit 0 (V_NOTRACE) compiles the barrier-timeline instrumentation out.  The launcher picks it whenever no
-// trace buffer is attached (-3.6 %: 905 vs 938 us per step, profiles/r2a_variants.md).  Round 1 left five more hand-over variants
+// trace buffer is attached.  Round 1 left five more hand-over variants
 // here (relaxed barriers over tagged activations, per-head readiness counters, a 4-way sharded barrier counter, producer-only
 // arrival, several steps per launch) and a third-generation kernel (attention fused with its out-projection); measured in round 2
-// they were bit-exact and 0.1 % faster to 11 % slower than this one, so they are gone (history: commit c3ab1ae).
+// they were bit-exact and no faster than this one, so they are gone (history: commit c3ab1ae).
 constexpr unsigned V_NOTRACE = 1;
 
 __device__ __noinline__ void wait_timeout(const char* what, unsigned a0, unsigned a1) {
@@ -94,7 +93,7 @@ struct GridBar {
 struct GemvDesc {
   const bf16* W;
   const float* bias;
-  int N, K, R;            // R rows per warp (1, 2 or 3)
+  int N, K, R;            // R rows per warp (1 .. RMAX)
   int n0, nend;           // rows of this CTA: [n0, nend), contiguous, ceil(N / CTAs) each (the LM head streams: [0, N))
   bool lm;
   const float* src;       // [M][K] fp32 activations written by an earlier phase
@@ -295,16 +294,16 @@ __device__ __forceinline__ void stage_x(float* xs, float* red, const GemvDesc& d
   else __syncthreads();
 }
 
-// lanes [8r, 8r + MB) finish row n + r  (R <= 3, MB <= 8)
+// lanes [8r, 8r + MB) finish row n + r  (R <= RMAX = 4, MB <= 8)
 template <int MB, unsigned VAR>
-__device__ __forceinline__ void finish_rows(const GemvDesc& d, const float (&acc)[3][MB], float bias, int n, int M, float res,
+__device__ __forceinline__ void finish_rows(const GemvDesc& d, const float (&acc)[RMAX][MB], float bias, int n, int M, float res,
                                             bool res_valid, int D, int Tmax, int pos, int lane) {
   const int m = lane & 7, r_sel = lane >> 3;
   const int nn = n + r_sel;
   if (r_sel < d.R && m < MB && m < M && nn < d.nend) {
     float v = 0.f;
 #pragma unroll
-    for (int r = 0; r < 3; ++r) {
+    for (int r = 0; r < RMAX; ++r) {
 #pragma unroll
       for (int mm = 0; mm < MB; ++mm)
         if (r == r_sel && mm == m) v = acc[r][mm];
@@ -438,8 +437,9 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
         mbar_wait(&cbar[ph & 1], (ph & 1) ? cpar1 : cpar0);
         if (mkbase && lane == 0) wts[warp][0] = global_ns();
         const uint8_t* slab = pool + ((ph & 1) ? 0 : a.p0_off) + (size_t)warp * cur.R * cur.K * 2;
-        float acc[3][MB];
-        if (cur.R == 3) dot_rows<MB, 3>(slab, xs, cur.K, acc, lane);
+        float acc[RMAX][MB];
+        if (cur.R == 4) dot_rows<MB, 4>(slab, xs, cur.K, acc, lane);
+        else if (cur.R == 3) dot_rows<MB, 3>(slab, xs, cur.K, acc, lane);
         else if (cur.R == 2) dot_rows<MB, 2>(slab, xs, cur.K, acc, lane);
         else dot_rows<MB, 1>(slab, xs, cur.K, acc, lane);
         finish_rows<MB, VAR>(cur, acc, pre.bias, n, Q, res, true, D, a.Tmax, pos, lane);
@@ -634,7 +634,7 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
         mbar_wait(&wbar[MW + warp], wpar1);
         wpar1 ^= 1u;
       }
-      float acc[3][MB];
+      float acc[RMAX][MB];
       dot_rows<MB, 2>(pool + buf * set_bytes + (size_t)warp * slab_bytes, xs, K, acc, lane);
       finish_rows<MB, VAR>(cur, acc, 0.f, n, Q, 0.f, true, D, a.Tmax, pos, lane);
       if (a.fuse_select) {
@@ -712,9 +712,9 @@ int launch_decode_mega(cudaStream_t st, const MegaArgs& a, int num_sms) {
   if (a.L > MEGA_MAXL || Q > 2 || a.D > MAXD || a.ffn > 5120 || a.D % 8 != 0 || a.ffn % 8 != 0 || a.Tmax > MAXKEYS) return -3;
   if ((size_t)MW * a.D * 2 > (size_t)ATT_OFF) return -3;  // R=1 slabs must stay below the attention scratch
   const long long GW = (long long)num_sms * MW;
-  {  // every layer GEMV is one pass of at most 3 rows per warp
+  {  // every layer GEMV is one pass of at most RMAX rows per warp
     const int nmax = 3 * a.D > a.ffn ? 3 * a.D : a.ffn;
-    if (((nmax + num_sms - 1) / num_sms + MW - 1) / MW > 3) return -3;
+    if (((nmax + num_sms - 1) / num_sms + MW - 1) / MW > RMAX) return -3;
   }
   (void)GW;
   if (a.nsplit > XSPLIT) return -3;
@@ -726,7 +726,7 @@ int launch_decode_mega(cudaStream_t st, const MegaArgs& a, int num_sms) {
   const int ks = (a.S + a.nsplit - 1) / a.nsplit;
   if (ks > XKMAX) return -3;
   BW_CUDA_OK(cudaMemsetAsync(a.bar, 0, 1024 * sizeof(unsigned), st));
-  // Co-residency of the 148 CTAs (round-1 advisor): the grid barriers spin, so a CTA that is not scheduled deadlocks the rest until
+  // Co-residency of the CTAs (one per SM) (round-1 advisor): the grid barriers spin, so a CTA that is not scheduled deadlocks the rest until
   // the 2^32-cycle timeout traps.  (1) the occupancy calculator must promise one CTA per SM, else -3 (per-op path); (2) the launch is
   // cooperative, so the driver either runs the whole grid at once or fails the launch (another kernel holding SMs: an error code at
   // the C-ABI, not a poisoned context).  BW_MEGA_COOP=0 falls back to the plain launch of round 1.

@@ -13,6 +13,7 @@ namespace mega {
 
 constexpr int MT = 384;        // threads per CTA (12 warps: <= 170 registers per thread)
 constexpr int MW = MT / 32;    // warps per CTA
+constexpr int RMAX = 4;        // weight rows per warp in a GEMV phase: row r is finished by lanes [8r, 8r + MB)
 constexpr int DMA_T = MT - 32;  // first lane of the last warp: issues every TMA operation (it takes no part in x staging)
 constexpr int KG = MT / 8;     // key groups of 8 lanes in the attention phases
 constexpr int MAXKEYS = 448;   // self-attention keys held in smem (Tmax)
@@ -100,7 +101,7 @@ __device__ __forceinline__ void dot_chunk(const uint8_t* slab, const float* xs, 
 // guard per chunk the compiler serialised load -> convert -> FMA chunk by chunk, ~120 cycles each); a ragged tail
 // (K % 256 != 0: only the small test models) takes the guarded path.
 template <int MB, int R>
-__device__ __forceinline__ void dot_rows(const uint8_t* slab, const float* xs, int K, float (&acc)[3][MB], int lane) {
+__device__ __forceinline__ void dot_rows(const uint8_t* slab, const float* xs, int K, float (&acc)[RMAX][MB], int lane) {
   float s[R][MB];
 #pragma unroll
   for (int r = 0; r < R; ++r)
@@ -112,7 +113,7 @@ __device__ __forceinline__ void dot_rows(const uint8_t* slab, const float* xs, i
   for (int c = 0; c < nfull; ++c, k0 += 256) dot_chunk<MB, R>(slab, xs, K, k0, true, s);
   if (k0 < K) dot_chunk<MB, R>(slab, xs, K, k0, (k0 + 128) < K, s);
 #pragma unroll
-  for (int r = 0; r < 3; ++r)
+  for (int r = 0; r < RMAX; ++r)
 #pragma unroll
     for (int m = 0; m < MB; ++m) acc[r][m] = (r < R) ? warp_sum(s[r < R ? r : 0][m]) : 0.f;
 }

@@ -4,8 +4,7 @@
 // At batch 1 every one of these moves only 3-13 MB, i.e. ~20-90 KB per SM: they are bound by DRAM *latency*, not
 // bandwidth, unless every byte a CTA needs is requested up front.  So each kernel issues ALL of its 16-byte weight / KV
 // loads into registers first (one DRAM round trip), overlaps the x staging + LayerNorm prologue with them, and only
-// then computes.  (First version looped load->use with 4-8 loads in flight: 3.0 ms per step, 10% of the HBM roofline;
-// see profiles/.)
+// then computes.  (A first version looped load->use with 4-8 loads in flight and reached a small fraction of the HBM roofline.)
 #include <math.h>
 
 #include "decode.cuh"
@@ -35,7 +34,7 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 
 // 8 consecutive values of a row that may be stored as nsplit raw split-K partial sums ([split][row][col], split_stride apart):
 // summed in split order (deterministic), + bias, * alpha.  The loads of four splits are issued together: a dependent
-// load -> add -> load chain costs one L2 round trip per split (96 us for the self-attention kernel at Q = 64: profiles/r2c).
+// load -> add -> load chain costs one L2 round trip per split.
 __device__ __forceinline__ void split_sum8(const float* __restrict__ p, long long idx, int nsplit, long long split_stride,
                                            const float* __restrict__ bias, int bias_idx, float alpha, float (&o)[8]) {
   float4 a0 = *reinterpret_cast<const float4*>(p + idx), a1 = *reinterpret_cast<const float4*>(p + idx + 4);
@@ -257,8 +256,8 @@ __device__ __forceinline__ float block_sum4(float v, float* red4) {
 // ------------------------------------------------------------------------------------------------
 // causal self-attention over cached positions 0..pos of one (sequence, head).  128 threads = 16 key groups x 8 lanes;
 // a lane owns 8 of the 64 head dims, so one warp-load covers 4 whole 128-byte K (or V) rows.  Keys are walked in chunks of 128
-// with an online softmax: 33 KB of static smem whatever Tmax is (the first version held all Tmax = 448 positions: 116 KB, ONE CTA
-// per SM, 43 waves at 320 sequences x 20 heads = 362 us per layer, profiles/r2c_summary.md); all loads of a chunk in flight together.
+// with an online softmax: 33 KB of static smem whatever Tmax is (holding all Tmax = 448 positions takes 116 KB: ONE CTA per SM);
+// all loads of a chunk in flight together.
 // ------------------------------------------------------------------------------------------------
 constexpr int SCH = 128;
 
@@ -531,7 +530,7 @@ __global__ void __launch_bounds__(128) cross_attn_kernel(const CrossAttnArgs a) 
 // ------------------------------------------------------------------------------------------------
 // Cross-attention for large batches: ONE CTA streams all S keys of one (audio, head) through a double-buffered smem ring with an
 // online softmax -- no key splits, so no partial results, no atomics, no __threadfence and no merge pass (the split kernel above
-// spends ~45 % of its issue slots on those and on block reductions at A = 64: profiles/r2a_summary.md, 0.68 of the HBM peak).
+// spends much of its issue slots on those and on block reductions at large A).
 // Chosen when A * H CTAs fill the machine at least twice; small batches keep the split kernel (more CTAs per byte).
 //   QK : thread t owns key t of the 128-key tile: its 128-byte K row sits in smem with the 16-byte pieces XOR-swizzled by (row & 7),
 //        so a row-per-thread LDS.128 is conflict-free; 64 FMAs per beam, no shuffles

@@ -1,11 +1,10 @@
-// Weight-streaming tcgen05 GEMM of the batched decoder step (q_len = 1 for Q sequences): out[q, n] = sum_k X[q, k] * W[n, k].
+// Weight-streaming wgmma GEMM of the batched decoder step (q_len = 1 for Q sequences): out[q, n] = sum_k X[q, k] * W[n, k].
 //
 // Shape of the problem: W is 3-13 MB and read once per step, X is Q x K with Q = 3..320 rows.  The step runs ~190 of these per
-// token, so what matters is the LATENCY of one launch, not its peak rate: measured with the generic kernel (128-row activation
-// tile, 32-column weight tile, 8-stage ring: profiles/r2b_summary.md) every projection took 12-23 us for 3-13 MB -- a CTA walked
-// 20-80 k-blocks through an 8-deep ring, i.e. 3-10 dependent DRAM round trips.  Here the operands are swapped and K is split:
-//   * the WEIGHT tile is the 128-row M operand of the MMA, the activations are the N operand (Q rounded up to 16, <= 256):
-//     a k-block costs 16 KB of W + Q x 128 B of X instead of 16 KB of zero-padded X + 4 KB of W, so 5-7 k-blocks fit in smem at once;
+// token, so what matters is the LATENCY of one launch, not its peak rate: a generic kernel (128-row activation tile, 32-column weight
+// tile, deep ring) walks 20-80 k-blocks per CTA, i.e. several dependent DRAM round trips.  Here the operands are swapped and K is split:
+//   * the WEIGHT tile is the 128-row M side of the MMA (two consumer warpgroups of 64 rows), the activations are the N side (Q rounded
+//     up to a wgmma width of 32, 64, 128 or 256): a k-block costs 16 KB of W + QB x 128 B of X, so several k-blocks fit in smem at once;
 //   * grid = (N / 128) x q-tiles x ksplit with ksplit the smallest count that gives >= 64 CTAs and lets a CTA's k-blocks fit its
 //     ring: every byte a CTA needs is requested by ONE thread before anything is awaited -- one DRAM round trip per launch;
 //   * under programmatic dependent launch the weight boxes are requested BEFORE griddepcontrol.wait (weights do not depend on the
@@ -13,8 +12,7 @@
 //   * split-K partial sums are written raw (fp32, [split][q][n]) and added by the consumer in a fixed order (resid_ln, the
 //     attention kernels' q/k/v loads, gelu_bias): deterministic, no atomics; ksplit = 1 launches (LM head) apply bias / alpha /
 //     GELU here and may write bf16.
-// Epilogue: TMEM lane = weight row n, column = sequence q, so for a fixed q the 32 lanes of a warp store 32 consecutive n: 128-byte
-// coalesced stores of the transposed tile.
+// Epilogue: accumulator row = weight row n, column = sequence q, so for a fixed q the 8 row-groups of a warp store 8 consecutive n.
 #include <limits.h>
 
 #include "kernels.h"
@@ -28,10 +26,11 @@ constexpr int DK = 64;
 constexpr int W_STAGE_BYTES = DM * DK * 2;  // 16 KB
 constexpr int MAX_STAGES = 8;
 constexpr int SMEM_BUDGET = 200 * 1024;
+constexpr int THREADS = 288;  // two consumer warpgroups + one TMA producer warp
+constexpr int CONSUMER_WARPS = 8;
 
 struct DecParams {
   int Q, N, K;
-  int QB;       // activation rows per q-tile (multiple of 16, <= 256) = MMA N
   int stages;   // ring depth (<= MAX_STAGES)
   int kper;     // k-blocks per split
   int n_store;  // columns n >= n_store are not written (weight rows that do not exist: tied LM head)
@@ -39,55 +38,38 @@ struct DecParams {
   GemmEpi epi;  // bias / alpha / act / out_f32 / out_bf16 / row_stride (= ldo); batch/head strides unused
 };
 
-__device__ __forceinline__ void umma_bf16_n(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-__global__ void __launch_bounds__(192, 1)
+template <int QB>
+__global__ void __launch_bounds__(THREADS, 1)
 gemm_dec_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const DecParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int x_stage_bytes = p.QB * DK * 2;
-  const int stage_bytes = W_STAGE_BYTES + ((x_stage_bytes + 1023) & ~1023);  // both operands 1024-byte aligned (128 B swizzle atoms)
+  constexpr int x_stage_bytes = QB * DK * 2;
+  constexpr int stage_bytes = W_STAGE_BYTES + ((x_stage_bytes + 1023) & ~1023);  // both operands 1024-byte aligned (128 B swizzle atoms)
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + MAX_STAGES;
-  uint64_t* accum_full = bars + 2 * MAX_STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * MAX_STAGES + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n0 = blockIdx.x * DM;
-  const int q0 = blockIdx.y * p.QB;
+  const int q0 = blockIdx.y * QB;
   const int nk_all = p.K / DK;
   const int kb0 = (int)blockIdx.z * p.kper;
   const int nk = min(nk_all, kb0 + p.kper) - kb0;
-  uint32_t tmem_cols = 32;
-  while ((int)tmem_cols < p.QB) tmem_cols <<= 1;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], CONSUMER_WARPS);
     }
-    mbar_init(accum_full, 1);
     fence_mbar_init();
   }
-  if (warp == 4 && lane == 0) {
+  if (warp == CONSUMER_WARPS && lane == 0) {
     tma_prefetch_desc(&tmW);
     tma_prefetch_desc(&tmX);
   }
-  if (warp == 5) tmem_alloc(tmem_slot, tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 4) {
+  if (warp == CONSUMER_WARPS) {
     if (lane == 0) {
       const int npre = nk < p.stages ? nk : p.stages;
       for (int kb = 0; kb < npre; ++kb) {  // weights: before the programmatic-launch wait
@@ -99,68 +81,72 @@ gemm_dec_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
       for (int kb = 0; kb < nk; ++kb) {
         const int s = kb % p.stages;
         if (kb >= npre) {
-          mbar_wait(&empty[s], ((kb / p.stages) & 1) ^ 1);
+          mbar_wait_wg(&empty[s], ((kb / p.stages) & 1) ^ 1);
           mbar_arrive_expect_tx(&full[s], W_STAGE_BYTES + x_stage_bytes);
           tma_load_2d(smem + (size_t)s * stage_bytes, &tmW, &full[s], (kb0 + kb) * DK, n0);
         }
         tma_load_2d(smem + (size_t)s * stage_bytes + W_STAGE_BYTES, &tmX, &full[s], (kb0 + kb) * DK, q0);
       }
     }
-  } else if (warp == 5) {
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_bf16(DM, p.QB);
-      for (int kb = 0; kb < nk; ++kb) {
-        const int s = kb % p.stages;
-        mbar_wait(&full[s], (kb / p.stages) & 1);
-        tc_fence_after();
-        const uint64_t a0 = umma_desc_sw128(smem_u32(smem + (size_t)s * stage_bytes));
-        const uint64_t b0 = umma_desc_sw128(smem_u32(smem + (size_t)s * stage_bytes + W_STAGE_BYTES));
+    return;
+  }
+  // ---------------- consumer warpgroup g: weight rows [n0 + 64 g, +64) ----------------
+  const int g = warp >> 2;
+  float acc[QB / 2];
 #pragma unroll
-        for (int k = 0; k < DK / 16; ++k) umma_bf16_n(tmem_base, a0 + 2 * k, b0 + 2 * k, idesc, (uint32_t)((kb | k) != 0));
-        umma_commit(&empty[s]);
-      }
-      umma_commit(accum_full);
-    }
-  } else {
-    // ---------------- epilogue: lane = weight row, TMEM column = sequence ----------------
-    pdl_wait();
-    const GemmEpi& e = p.epi;
-    const int n = n0 + warp * 32 + lane;
-    const bool n_ok = n < p.n_store;
-    const float bias = (e.bias && n_ok) ? e.bias[n] : 0.f;
+  for (int i = 0; i < QB / 2; ++i) acc[i] = 0.f;
+  for (int kb = 0; kb < nk; ++kb) {
+    const int s = kb % p.stages;
+    mbar_wait_wg(&full[s], (kb / p.stages) & 1);
+    wg_fence();
+    uint8_t* st = smem + (size_t)s * stage_bytes;
+    wg_kblock<QB>(acc, smem_u32(st + g * (W_STAGE_BYTES / 2)), smem_u32(st + W_STAGE_BYTES));
+    wg_commit();
+    wg_wait<1>();
+    if (kb > 0 && lane == 0) mbar_arrive(&empty[(kb - 1) % p.stages]);
+  }
+  wg_wait<0>();
+  wg_pin(acc);
+
+  // ---------------- epilogue: this thread holds weight rows n and n + 8, two adjacent sequences of every 8 ----------------
+  pdl_wait();
+  const GemmEpi& e = p.epi;
+  const int qn = min(QB, p.Q - q0);  // valid sequences of this q-tile
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int n = n0 + g * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+    if (n >= p.n_store) continue;
+    const float bias = e.bias ? e.bias[n] : 0.f;
     const float alpha = (n < e.alpha_cols) ? e.alpha : 1.0f;
-    mbar_wait(accum_full, 0);
-    tc_fence_after();
-    const uint32_t trow = tmem_base + ((uint32_t)(warp * 32) << 16);
-    const int qn = min(p.QB, p.Q - q0);  // valid sequences of this q-tile
     float* of = e.out_f32 ? e.out_f32 + (long long)blockIdx.z * p.split_stride + n : nullptr;
     bf16* ob = e.out_bf16 ? e.out_bf16 + n : nullptr;
-#pragma unroll 1
-    for (int c = 0; c * 32 < qn; ++c) {
-      uint32_t v[32];
-      tmem_ld_32x32(trow + c * 32, v);
-      tmem_ld_wait();
-      if (n_ok) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int q = c * 32 + j;
-          if (q < qn) {
-            float f = (__uint_as_float(v[j]) + bias) * alpha;
-            if (e.act == 1) f = gelu_erf(f);
-            const long long off = (long long)(q0 + q) * e.row_stride;
-            if (of) of[off] = f;
-            else ob[off] = f2e(f);
-          }
+    for (int j = 0; j < QB / 8; ++j) {
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const int q = 8 * j + 2 * (lane & 3) + c;
+        if (q < qn) {
+          float f = (acc[4 * j + 2 * h + c] + bias) * alpha;
+          if (e.act == 1) f = gelu_erf(f);
+          const long long off = (long long)(q0 + q) * e.row_stride;
+          if (of) of[off] = f;
+          else ob[off] = f2e(f);
         }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    __syncwarp();
-    tmem_dealloc(tmem_base, tmem_cols);
+}
+
+template <int QB>
+int launch_dec(cudaStream_t st, const CUtensorMap& tmW, const CUtensorMap& tmX, const DecParams& p, const DecGemmPlan& pl) {
+  static size_t attr = 0;
+  if (pl.smem > attr) {
+    BW_CUDA_OK(cudaFuncSetAttribute(gemm_dec_kernel<QB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
+    attr = pl.smem;
   }
+  dim3 grid((p.N + DM - 1) / DM, pl.q_tiles, pl.ksplit);
+  BW_CUDA_OK(launch_k(gemm_dec_kernel<QB>, grid, dim3(THREADS), pl.smem, st, tmW, tmX, p));
+  return 0;
 }
 
 // h[q, n] = bf16( GELU( sum_s part[s][q][n] + bias[n] ) ): the consumer of fc1's split-K partial sums (operand of fc2)
@@ -190,14 +176,16 @@ __global__ void __launch_bounds__(256) gelu_bias_kernel(const float* __restrict_
 DecGemmPlan gemm_dec_plan(int Q, int N, int K, int num_sms, bool want_split) {
   DecGemmPlan pl;
   pl.q_tiles = (Q + 255) / 256;
-  pl.QB = ((Q + pl.q_tiles - 1) / pl.q_tiles + 15) / 16 * 16;
+  const int per_tile = (Q + pl.q_tiles - 1) / pl.q_tiles;
+  pl.QB = 32;  // a wgmma width: 32, 64, 128 or 256
+  while (pl.QB < per_tile) pl.QB <<= 1;
   const int stage_bytes = W_STAGE_BYTES + ((pl.QB * DK * 2 + 1023) & ~1023);
   pl.stages = SMEM_BUDGET / stage_bytes;
   if (pl.stages > MAX_STAGES) pl.stages = MAX_STAGES;
   const int nk = K / DK;
   const int n_tiles = (N + DM - 1) / DM;
   // as few splits as give (a) a CTA all of its k-blocks in one ring pass and (b) >= 64 CTAs: every extra split is another partial-sum
-  // row the consumer has to read (10-14 splits made resid_ln 9.5 us: profiles/r2c_summary.md)
+  // row the consumer has to read
   int ks = 1;
   if (want_split) {
     const int ctas1 = n_tiles * pl.q_tiles;
@@ -220,22 +208,21 @@ int gemm_dec(cudaStream_t st, const bf16* X, const bf16* W, int Q, int N, int K,
   BW_CHECK(K % DK == 0 && K >= DK, "gemm_dec: K=%d must be a multiple of 64", K);
   BW_CHECK((epi.out_f32 != nullptr) != (epi.out_bf16 != nullptr), "gemm_dec: exactly one of out_f32/out_bf16 must be set");
   BW_CHECK(pl.ksplit == 1 || (epi.out_f32 && !epi.bias && epi.act == 0 && epi.alpha == 1.0f), "gemm_dec: split-K writes raw fp32 partial sums");
-  BW_CHECK(pl.QB % 16 == 0 && pl.QB >= 16 && pl.QB <= 256 && pl.stages >= 2, "gemm_dec: bad plan (QB=%d stages=%d)", pl.QB, pl.stages);
+  BW_CHECK((pl.QB == 32 || pl.QB == 64 || pl.QB == 128 || pl.QB == 256) && pl.stages >= 2 && pl.stages <= MAX_STAGES,
+           "gemm_dec: bad plan (QB=%d stages=%d)", pl.QB, pl.stages);
   CUtensorMap tmW, tmX;
   const int w_rows = (n_valid > 0 && n_valid < N) ? n_valid : N;
   if (int rc = make_tmap_2d_bf16(&tmW, W, (uint64_t)w_rows, (uint64_t)K, (uint64_t)K * 2, DM, DK)) return rc;
   if (int rc = make_tmap_2d_bf16(&tmX, X, (uint64_t)Q, (uint64_t)K, (uint64_t)K * 2, (uint32_t)pl.QB, DK)) return rc;
-  static size_t attr = 0;
-  if (pl.smem > attr) {
-    BW_CUDA_OK(cudaFuncSetAttribute(gemm_dec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
-    attr = pl.smem;
-  }
   DecParams p;
-  p.Q = Q; p.N = N; p.K = K; p.QB = pl.QB; p.stages = pl.stages; p.kper = pl.kper; p.n_store = w_rows; p.split_stride = split_stride;
+  p.Q = Q; p.N = N; p.K = K; p.stages = pl.stages; p.kper = pl.kper; p.n_store = w_rows; p.split_stride = split_stride;
   p.epi = epi;
-  dim3 grid((N + DM - 1) / DM, pl.q_tiles, pl.ksplit);
-  BW_CUDA_OK(launch_k(gemm_dec_kernel, grid, dim3(192), pl.smem, st, tmW, tmX, p));
-  return 0;
+  switch (pl.QB) {
+    case 32: return launch_dec<32>(st, tmW, tmX, p, pl);
+    case 64: return launch_dec<64>(st, tmW, tmX, p, pl);
+    case 128: return launch_dec<128>(st, tmW, tmX, p, pl);
+    default: return launch_dec<256>(st, tmW, tmX, p, pl);
+  }
 }
 
 int launch_gelu_bias(cudaStream_t st, const float* part, int nsplit, long long split_stride, const float* bias, bf16* h, int Q, int N) {

@@ -1,15 +1,19 @@
-// tcgen05 / TMEM / TMA GEMM for sm_100a:  C[b,t,n] = epi( sum_k A(b,t,k) * W[n,k] ).
+// wgmma / TMA GEMM for sm_90a:  C[b,t,n] = epi( sum_k A(b,t,k) * W[n,k] ).
 //
 // Replaces the cuBLAS GEMMs + cuDNN convs the reference reaches through torch
 // (TF/models/whisper/modeling_whisper.py:279-336 q/k/v/out projections, :404-407 fc1/fc2, :619-620 conv stem).
 //
-// Structure (one 128 x BN output tile per CTA, 192 threads):
-//   warps 0-3  epilogue: tcgen05.ld accumulator rows -> bias/alpha/GELU/pos/residual -> vectorised st.global
-//   warp  4    TMA producer (one lane): 128B-swizzled K-major boxes of A (3-D map, wrapping k for the conv
+// Structure (one 128 x BN output tile per CTA, 288 threads):
+//   warps 0-7  two consumer warpgroups: warpgroup g issues 4 x wgmma m64nBNk16 per 64-wide k-block for tile rows [64 g, 64 g + 64),
+//              keeps one k-block in flight and hands the previous smem stage back; the epilogue (bias/alpha/GELU/pos/residual)
+//              runs on the accumulator registers
+//   warp  8    TMA producer (one lane): 128B-swizzled K-major boxes of A (3-D map, wrapping k for the conv
 //              stem) and W into a STAGES-deep smem ring, completion on mbarriers
-//   warp  5    TMEM allocator + MMA issuer (one lane): 4 x tcgen05.mma (K=16) per 64-wide k-block,
-//              tcgen05.commit releases the smem stage / signals the epilogue
-// BN=128 uses 3 stages (96 KB) so two CTAs share an SM and one CTA's epilogue overlaps the other's main loop.
+// Tiles walk n-fastest (blockIdx.x): the CTAs running together work on a few 128-row bands of A against all of W (<= 13 MB:
+// L2-resident), so A streams from DRAM about once.
+// gemm_tc2 runs the same kernel over the encoder's activations of all B items as ONE [B * rows, K] matrix (no per-item tail tiles:
+// 1500 rows per item leave a 92-row tail); its epilogue maps the flat row r back to b = r / rows_per_item, t = r % rows_per_item,
+// and is compiled once per combination the encoder uses (MODE) with the 2-MUFU GELU below.
 #include <limits.h>
 
 #include "kernels.h"
@@ -21,21 +25,26 @@ namespace {
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
+constexpr int THREADS = 288;
+constexpr int CONSUMER_WARPS = 8;
 
 // BN = 32 is the decoder-step shape (q_len = 1 for up to 128 sequences per tile): the GEMM is a stream over the weight matrix, so
-// the tile is narrow (N / 32 CTAs cover the SMs without split-K for N >= 3840) and the ring is deep (8 stages x 20 KB in
-// flight per SM hide the DRAM latency; one CTA per SM).
+// the tile is narrow (N / 32 CTAs cover the SMs without split-K for N >= 3840) and the ring is deep (8 stages x 20 KB in flight per SM
+// hide the DRAM latency).  Wider tiles take as many stages as fit in 227 KB of shared memory.
 template <int BN>
 struct Cfg {
-  static constexpr int STAGES = (BN == 128) ? 3 : (BN == 32) ? 8 : 4;
+  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128) ? 6 : 8;
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
-  static constexpr int TMEM_COLS = (BN < 32) ? 32 : BN;  // power of two >= 32
   static constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + 1024 /*align slack*/ + 256 /*barriers*/;
-  static constexpr int MIN_CTAS = (BN == 256 || BN == 32) ? 1 : 2;
 };
+
+// epilogue specialisations: the runtime-parameterised generic one executes every option's instructions predicated off
+enum { EPI_GENERIC = 0, EPI_GELU = 1 /* bias, GELU -> 16 bit */, EPI_RESID = 2 /* bias, + fp32 residual -> fp32 */, EPI_PLAIN = 3 /* bias -> 16 bit */ };
 
 struct GemmParams {
   int B, rows, N, K;
+  int rows_per_item = INT_MAX;  // epilogue address map of a flat launch (B = 1): b = t / rows_per_item, t = t % rows_per_item
+  int fast_gelu = 0;            // GELU through gelu_as (gemm_tc2) instead of erff
   int kwrap;
   int tiles_m;  // per item
   int ksplit;   // gridDim.z: split z handles k-blocks [z * kper, min(nk, (z + 1) * kper)) and writes its partial sums at
@@ -52,8 +61,23 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-template <int BN>
-__global__ void __launch_bounds__(192, Cfg<BN>::MIN_CTAS)
+// exact (erf) GELU to 4e-7 absolute: Phi(x) through Abramowitz-Stegun 7.1.26 (|erf error| <= 1.5e-7) -- 2 MUFU + 12 fp32 operations where erff
+// costs ~25; the result is rounded to 16 bits right after (half an ulp there is >= 2.4e-4 relative).  tests/test_ops_gpu.py pins it to erf.
+__device__ __forceinline__ float gelu_as(float x) {
+  const float ax = fabsf(x);
+  float t;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(fmaf(0.3275911f * 0.70710678f, ax, 1.0f)));
+  float q = 0.5f * 1.061405429f;
+  q = fmaf(q, t, 0.5f * -1.453152027f);
+  q = fmaf(q, t, 0.5f * 1.421413741f);
+  q = fmaf(q, t, 0.5f * -0.284496736f);
+  q = fmaf(q, t, 0.5f * 0.254829592f);
+  q = (q * t) * ex2_approx((x * -0.72134752f) * x);  // 0.5 erfc(|x| / sqrt 2) = Phi(-|x|)
+  return fmaf(-ax, q, fmaxf(x, 0.f));               // x >= 0: x - x q;  x < 0: x q
+}
+
+template <int BN, int MODE>
+__global__ void __launch_bounds__(THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const GemmParams p) {
   using C = Cfg<BN>;
   extern __shared__ uint8_t smem_raw[];
@@ -63,8 +87,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint64_t* bars = reinterpret_cast<uint64_t*>(sB + C::STAGES * C::B_STAGE_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + C::STAGES;
-  uint64_t* accum_full = bars + 2 * C::STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * C::STAGES + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -78,22 +100,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (threadIdx.x == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], CONSUMER_WARPS);
     }
-    mbar_init(accum_full, 1);
     fence_mbar_init();
   }
-  if (warp == 4 && lane == 0) {
+  if (warp == CONSUMER_WARPS && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmW);
   }
-  if (warp == 5) tmem_alloc(tmem_slot, C::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 4) {
+  if (warp == CONSUMER_WARPS) {
     if (lane == 0) {
       // The weight tiles of the first ring pass do not depend on the previous kernel: under programmatic dependent launch they are
       // requested before the wait (their DRAM latency runs beside the predecessor's tail); the activations after it.
@@ -109,107 +126,75 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const uint32_t ph = (kb / C::STAGES) & 1;
         const int k = (kb0 + kb) * BK;
         if (kb >= npre) {
-          mbar_wait(&empty[s], ph ^ 1);
+          mbar_wait_wg(&empty[s], ph ^ 1);
           mbar_arrive_expect_tx(&full[s], A_STAGE_BYTES + C::B_STAGE_BYTES);
           tma_load_2d(sB + s * C::B_STAGE_BYTES, &tmW, &full[s], k, n0);
         }
         tma_load_3d(sA + s * A_STAGE_BYTES, &tmA, &full[s], k % p.kwrap, t0 + k / p.kwrap, b);
       }
     }
-  } else if (warp == 5) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(BM, BN);
-      for (int kb = 0; kb < nk; ++kb) {
-        const int s = kb % C::STAGES;
-        const uint32_t ph = (kb / C::STAGES) & 1;
-        mbar_wait(&full[s], ph);
-        tc_fence_after();
-        const uint64_t a0 = umma_desc_sw128(smem_u32(sA + s * A_STAGE_BYTES));
-        const uint64_t b0 = umma_desc_sw128(smem_u32(sB + s * C::B_STAGE_BYTES));
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k)  // +32 B per K=16 step inside the 128 B swizzle atom
-          umma_bf16(tmem_base, a0 + 2 * k, b0 + 2 * k, idesc, (uint32_t)((kb | k) != 0));
-        umma_commit(&empty[s]);
-      }
-      umma_commit(accum_full);
-    }
   } else {
-    // ---------------- epilogue: warp w owns TMEM lanes [32w, 32w+32) = tile rows ----------------
+    // ---------------- consumer warpgroup g: tile rows [64 g, 64 g + 64) ----------------
+    const int g = warp >> 2;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < nk; ++kb) {
+      const int s = kb % C::STAGES;
+      mbar_wait_wg(&full[s], (kb / C::STAGES) & 1);
+      wg_fence();
+      wg_kblock<BN>(acc, smem_u32(sA + s * A_STAGE_BYTES + g * (A_STAGE_BYTES / 2)), smem_u32(sB + s * C::B_STAGE_BYTES));
+      wg_commit();
+      wg_wait<1>();  // k-block kb - 1 is complete: its stage goes back to the producer
+      if (kb > 0 && lane == 0) mbar_arrive(&empty[(kb - 1) % C::STAGES]);
+    }
+    wg_wait<0>();
+    wg_pin(acc);
+
+    // ---------------- epilogue: this thread holds rows r and r + 8, two adjacent columns of every 8-column group ----------------
     pdl_wait();  // (residual reads / output stores: after the predecessor grid)
-    mbar_wait(accum_full, 0);
-    tc_fence_after();
-    const int t = t0 + warp * 32 + lane;
-    const bool row_ok = t < p.rows;
-    const uint32_t trow = tmem_base + ((uint32_t)(warp * 32) << 16);
     const GemmEpi& e = p.epi;
-    const long long row_off = (long long)b * e.batch_stride + (long long)t * e.row_stride + (long long)blockIdx.z * p.split_stride;
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      const int n = n0 + c * 32;
-      if (n >= p.N) break;  // warp-uniform
-      uint32_t v[32];
-      tmem_ld_32x32(trow + c * 32, v);
-      tmem_ld_wait();
-      if (row_ok) {
-        const long long off = row_off + (long long)(n >> 6) * e.head_stride + (n & 63);
-        float f[32];
+    constexpr bool GEN = MODE == EPI_GENERIC;
+    const bool do_alpha = GEN && e.alpha != 1.0f;
+    const bool do_act = GEN ? e.act == 1 : MODE == EPI_GELU;
+    const bool fast_gelu = GEN ? p.fast_gelu != 0 : true;
+    const bool has_pos = GEN && e.pos != nullptr;
+    const bool has_res = GEN ? e.residual != nullptr : MODE == EPI_RESID;
+    const bool f32out = GEN ? e.out_f32 != nullptr : MODE == EPI_RESID;
+    const int r = g * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-        for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
+    for (int h = 0; h < 2; ++h) {
+      const int t = t0 + r + 8 * h;
+      if (t >= p.rows) continue;
+      const int bi = t / p.rows_per_item, ti = t - bi * p.rows_per_item;  // (bi = 0 unless a flat launch)
+      const long long row_off = (long long)(b + bi) * e.batch_stride + (long long)ti * e.row_stride + (long long)blockIdx.z * p.split_stride;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = n0 + 8 * j + 2 * (lane & 3);
+        if (n >= p.N) break;  // N % 32 == 0: uniform over the 8 x 4 threads of a 32-column chunk
+        float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
         if (e.bias) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 bb = *reinterpret_cast<const float4*>(e.bias + n + j);
-            f[j] += bb.x; f[j + 1] += bb.y; f[j + 2] += bb.z; f[j + 3] += bb.w;
-          }
+          const float2 bb = __ldg(reinterpret_cast<const float2*>(e.bias + n));
+          f0 += bb.x; f1 += bb.y;
         }
-        if (e.alpha != 1.0f && n < e.alpha_cols) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] *= e.alpha;
+        if (do_alpha && n < e.alpha_cols) { f0 *= e.alpha; f1 *= e.alpha; }
+        if (do_act) {
+          if (fast_gelu) { f0 = gelu_as(f0); f1 = gelu_as(f1); }
+          else { f0 = gelu_erf(f0); f1 = gelu_erf(f1); }
         }
-        if (e.act == 1) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = gelu_erf(f[j]);
+        if (has_pos) {
+          const float2 q = *reinterpret_cast<const float2*>(e.pos + (long long)t * p.N + n);
+          f0 += q.x; f1 += q.y;
         }
-        if (e.pos) {
-          const float* pp = e.pos + (long long)t * p.N + n;
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 q = *reinterpret_cast<const float4*>(pp + j);
-            f[j] += q.x; f[j + 1] += q.y; f[j + 2] += q.z; f[j + 3] += q.w;
-          }
+        const long long off = row_off + (long long)(n >> 6) * e.head_stride + (n & 63);
+        if (has_res) {
+          const float2 q = *reinterpret_cast<const float2*>(e.residual + off);
+          f0 += q.x; f1 += q.y;
         }
-        if (e.residual) {
-          const float* rp = e.residual + off;
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 q = *reinterpret_cast<const float4*>(rp + j);
-            f[j] += q.x; f[j + 1] += q.y; f[j + 2] += q.z; f[j + 3] += q.w;
-          }
-        }
-        if (e.out_f32) {
-          float* op = e.out_f32 + off;
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(op + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-        } else {
-          bf16* op = e.out_bf16 + off;
-#pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            uint4 q;
-            q.x = pack_bf16(f[j], f[j + 1]);
-            q.y = pack_bf16(f[j + 2], f[j + 3]);
-            q.z = pack_bf16(f[j + 4], f[j + 5]);
-            q.w = pack_bf16(f[j + 6], f[j + 7]);
-            *reinterpret_cast<uint4*>(op + j) = q;
-          }
-        }
+        if (f32out) *reinterpret_cast<float2*>(e.out_f32 + off) = make_float2(f0, f1);
+        else *reinterpret_cast<uint32_t*>(e.out_bf16 + off) = pack_bf16(f0, f1);
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    __syncwarp();
-    tmem_dealloc(tmem_base, C::TMEM_COLS);
   }
 }
 
@@ -267,6 +252,16 @@ int check_epi(const GemmEpi& e, int N) {
 
 }  // namespace
 
+int device_sms() {
+  static int sms = 0;
+  if (sms == 0) {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) sms = n;
+    else return 132;  // H100 SXM
+  }
+  return sms;
+}
+
 int make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t row_pitch_bytes,
                       uint32_t box_rows, uint32_t box_cols) {
   EncodeTiledFn fn = get_encode_fn();
@@ -300,18 +295,18 @@ static int make_tmap_3d_bf16(CUtensorMap* out, const void* base, uint64_t batch,
   return 0;
 }
 
-template <int BN>
-static int launch_tc(cudaStream_t st, const CUtensorMap& tmA, const GemmA& a, const bf16* W, const GemmParams& p) {
+template <int BN, int MODE = EPI_GENERIC>
+static int launch_tc(cudaStream_t st, const CUtensorMap& tmA, const bf16* W, const GemmParams& p) {
   using C = Cfg<BN>;
   CUtensorMap tmW;
   if (int rc = make_tmap_2d_bf16(&tmW, W, p.epi.n_valid > 0 ? p.epi.n_valid : p.N, p.K, (uint64_t)p.K * 2, BN, BK)) return rc;
   static bool attr_set = false;
   if (!attr_set) {
-    BW_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+    BW_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     attr_set = true;
   }
   dim3 grid((p.N + BN - 1) / BN, p.tiles_m * p.B, p.ksplit);
-  BW_CUDA_OK(launch_k(gemm_tc_kernel<BN>, grid, dim3(192), (size_t)C::SMEM_BYTES, st, tmA, tmW, p));
+  BW_CUDA_OK(launch_k(gemm_tc_kernel<BN, MODE>, grid, dim3(THREADS), (size_t)C::SMEM_BYTES, st, tmA, tmW, p));
   return 0;
 }
 
@@ -353,18 +348,68 @@ int gemm_tc_split(cudaStream_t st, const GemmA& a, const bf16* W, int B, int row
     return rc;
   int bn = force_bn;
   if (bn == 0) {
-    // enough CTAs to cover the 148 SMs matters more than the wider tile when the grid is small
+    // enough CTAs to cover the SMs matters more than the wider tile when the grid is small
     const long long tiles128 = (long long)((N + 127) / 128) * p.tiles_m * B;
-    bn = (N % 256 == 0 && tiles128 >= 4 * 148) ? 256 : 128;
+    bn = (N % 256 == 0 && tiles128 >= 4 * device_sms()) ? 256 : 128;
     if (N < 128) bn = 64;
   }
   switch (bn) {
-    case 32: return launch_tc<32>(st, tmA, a, W, p);
-    case 64: return launch_tc<64>(st, tmA, a, W, p);
-    case 128: return launch_tc<128>(st, tmA, a, W, p);
-    case 256: return launch_tc<256>(st, tmA, a, W, p);
+    case 32: return launch_tc<32>(st, tmA, W, p);
+    case 64: return launch_tc<64>(st, tmA, W, p);
+    case 128: return launch_tc<128>(st, tmA, W, p);
+    case 256: return launch_tc<256>(st, tmA, W, p);
   }
   BW_CHECK(false, "gemm_tc: unsupported BN=%d", bn);
+}
+
+bool gemm_tc2_supported(int M, int N, int K) { return K % BK == 0 && K >= BK && (N % 256 == 0 || N % 128 == 0) && M >= 1; }
+
+int gemm_tc2(cudaStream_t st, const bf16* A, const bf16* W, int M, int N, int K, int rows_per_item, const GemmEpi& epi, int force_bn) {
+  BW_CHECK((epi.out_f32 != nullptr) != (epi.out_bf16 != nullptr), "gemm_tc2: exactly one of out_f32/out_bf16 must be set");
+  BW_CHECK(gemm_tc2_supported(M, N, K), "gemm_tc2: unsupported shape M=%d N=%d K=%d", M, N, K);
+  BW_CHECK(!epi.pos, "gemm_tc2: positional-table epilogue is not supported (conv stem stays on gemm_tc)");
+  BW_CHECK(epi.row_stride % 8 == 0 && epi.batch_stride % 8 == 0 && epi.head_stride % 8 == 0, "gemm_tc2: output strides must be multiples of 8");
+  GemmParams p;
+  p.B = 1; p.rows = M; p.N = N; p.K = K;
+  p.rows_per_item = rows_per_item > 0 ? rows_per_item : INT_MAX;
+  p.fast_gelu = 1;
+  p.kwrap = INT_MAX;
+  p.tiles_m = (M + BM - 1) / BM;
+  p.ksplit = 1; p.kper = K / BK; p.split_stride = 0;
+  p.epi = epi;
+  CUtensorMap tmA;
+  if (int rc = make_tmap_3d_bf16(&tmA, A, 1, (uint64_t)M, (uint64_t)K, (uint64_t)K * 2, (uint64_t)M * K * 2, BM, BK)) return rc;
+  int force_mode = -1;
+  if (force_bn >= 1000) {  // tests: 1000 + bn = the generic (runtime-parameterised) epilogue instead of the specialised one
+    force_mode = EPI_GENERIC;
+    force_bn -= 1000;
+  }
+  int bn = force_bn;
+  if (bn == 0) {
+    // 256-wide tiles halve the L2 traffic per MAC; fall back to 128 when 256 does not divide N or leaves the last wave thin
+    bn = (N % 256 == 0) ? 256 : 128;
+    if (bn == 256) {
+      const int sms = device_sms();
+      const long long t256 = (long long)p.tiles_m * (N / 256);
+      const long long waves = (t256 + sms - 1) / sms;
+      if (t256 * 10 < waves * sms * 8) bn = 128;  // < 80 % of the last wave's slots used
+    }
+  }
+  BW_CHECK(bn == 128 || bn == 256, "gemm_tc2: unsupported tile width %d", bn);
+  BW_CHECK(N % bn == 0, "gemm_tc2: N=%d is not a multiple of the tile width %d", N, bn);
+  int mode = EPI_GENERIC;
+  if (epi.alpha == 1.0f) {
+    if (epi.act == 1 && !epi.residual && epi.out_bf16) mode = EPI_GELU;
+    else if (epi.act == 0 && epi.residual && epi.out_f32) mode = EPI_RESID;
+    else if (epi.act == 0 && !epi.residual && epi.out_bf16) mode = EPI_PLAIN;
+  }
+  if (force_mode >= 0) mode = force_mode;
+#define BW_TC2_CASE(BNV, MODEV) \
+  if (bn == BNV && mode == MODEV) return launch_tc<BNV, MODEV>(st, tmA, W, p);
+  BW_TC2_CASE(256, EPI_GENERIC) BW_TC2_CASE(256, EPI_GELU) BW_TC2_CASE(256, EPI_RESID) BW_TC2_CASE(256, EPI_PLAIN)
+  BW_TC2_CASE(128, EPI_GENERIC) BW_TC2_CASE(128, EPI_GELU) BW_TC2_CASE(128, EPI_RESID) BW_TC2_CASE(128, EPI_PLAIN)
+#undef BW_TC2_CASE
+  BW_CHECK(false, "gemm_tc2: no kernel for bn=%d mode=%d", bn, mode);
 }
 
 int gemm_simt(cudaStream_t st, const GemmA& a, const bf16* W, int B, int rows, int N, int K, const GemmEpi& epi) {

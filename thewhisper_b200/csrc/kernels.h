@@ -5,7 +5,7 @@
 namespace BW_NS {
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05 GEMM: C[b,t,n] = epilogue( sum_k A(b,t,k) * W[n,k] ), bf16 operands, fp32 accumulate in TMEM
+// wgmma GEMM: C[b,t,n] = epilogue( sum_k A(b,t,k) * W[n,k] ), bf16 operands, fp32 accumulate in registers
 // ---------------------------------------------------------------------------------------------
 // A operand view.  Element (b, t, k) lives at base[b*batch_stride + (t + k / kwrap) * pitch + (k % kwrap)].
 //   plain row-major activations : kwrap >= K, pitch = row length
@@ -39,13 +39,13 @@ struct GemmEpi {
 
 // W: [N, K] bf16 row-major (torch Linear layout).  K % 64 == 0, N % 32 == 0.  rows = output rows per item.
 int gemm_tc(cudaStream_t st, const GemmA& a, const bf16* W, int B, int rows, int N, int K, const GemmEpi& epi,
-            int force_bn /*0 = auto, else 64/128/256*/);
-// Split-K form for the decoder's residual GEMMs (K >> N / 148 tiles): grid.z = ksplit, split z writes raw fp32 partial sums at
+            int force_bn /*0 = auto, else 32/64/128/256*/);
+// Split-K form for the decoder's residual GEMMs (K >> N / SM-count tiles): grid.z = ksplit, split z writes raw fp32 partial sums at
 // out_f32 + z * split_stride; the consumer (resid_ln) adds them in a fixed order.  ksplit is clamped so that every split owns a k-block (gemm_tc_ksplit gives the count used).
 int gemm_tc_split(cudaStream_t st, const GemmA& a, const bf16* W, int B, int rows, int N, int K, const GemmEpi& epi, int force_bn,
                   int ksplit, long long split_stride);
 int gemm_tc_ksplit(int K, int ksplit);
-// Second-generation encoder GEMM (gemm_tc2.cu): CTA pairs (cta_group::2, 256 x BN tiles), persistent, double-buffered TMEM.
+// Encoder GEMM over flat rows (the gemm_tc kernel, B = 1): 128 x BN tiles across item boundaries, epilogues specialised per use.
 // A [M, K] plain row-major; the epilogue address map splits the flat row r as b = r / rows_per_item, t = r % rows_per_item
 // (rows_per_item <= 0: one item).  No conv wrap, no positional table.  force_bn: 0 auto, 128, 256 (+ 1000: generic epilogue, tests).
 bool gemm_tc2_supported(int M, int N, int K);
@@ -73,9 +73,8 @@ int launch_gelu_bias(cudaStream_t st, const float* part, int nsplit, long long s
 // encoder attention (non-causal).  qkv: [B*S, 3*D] bf16 (q pre-scaled by dh^-1/2), vt: [B, H, 64, Spad] bf16
 // (zero beyond S), out: [B*S, D] bf16.  head_dim is 64 for every Whisper size.
 // ---------------------------------------------------------------------------------------------
+// same kernel; vt == nullptr reads V straight from the qkv rows (MN-major operand) instead of the transposed copy
 int attn_enc_tc(cudaStream_t st, const bf16* qkv, const bf16* vt, bf16* out, int B, int S, int Spad, int H);
-// second generation: two query tiles per CTA in ping-pong, O accumulated in TMEM with lazy rescaling (same arguments)
-int attn_enc_tc2(cudaStream_t st, const bf16* qkv, const bf16* vt, bf16* out, int B, int S, int Spad, int H);
 int attn_enc_simt(cudaStream_t st, const bf16* qkv, bf16* out, int B, int S, int H);
 int transpose_v(cudaStream_t st, const bf16* qkv, bf16* vt, int B, int S, int Spad, int H);
 

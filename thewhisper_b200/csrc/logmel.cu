@@ -1,4 +1,4 @@
-// Fused log-mel front end for sm_100a: reflect-pad framing + periodic Hann window + 400-point FFT + |.|^2 +
+// Fused log-mel front end for sm_90a: reflect-pad framing + periodic Hann window + 400-point FFT + |.|^2 +
 // sparse slaney mel filter bank + log10, then the per-sample dynamic-range clamp and (x+4)/4.
 //
 // Replaces WhisperFeatureExtractor._torch_extract_fbank_features, which the reference runs with torch.stft on the

@@ -1,4 +1,4 @@
-"""Host-side generation control for the B200 engine: prompt tokens, the short-form `seek` loop, segment
+"""Host-side generation control for the engine: prompt tokens, the short-form `seek` loop, segment
 extraction and token timestamps -- the integer/host half of WhisperGenerationMixin.generate
 (TF/models/whisper/generation_whisper.py:383-968), restated without torch modules.  All arithmetic (encoder,
 decoder steps, logits processors, argmax, DTW) runs in the CUDA engine; this module only sequences it.

@@ -1,5 +1,5 @@
 """Drop-in for `thestage_speechkit.nvidia.ASRPipeline` (REF thestage_speechkit/nvidia/asr_pipeline.py:30-92) on the
-B200-native engine.
+H100-native engine.
 
 Same constructor and call surface (SURVEY.md §8b): `ASRPipeline(model, feature_extractor=None, tokenizer=None,
 model_size=None, chunk_length_s=30, device="cuda", torch_dtype=None, batch_size=..., revision=...)` and
@@ -172,7 +172,7 @@ class ASRPipeline:
             raise ValueError("Whisper cannot return `char` timestamps, only word level or segment level timestamps. "
                              "Use `return_timestamps='word'` or `return_timestamps=True` respectively.")
         if generate_kwargs.get("do_sample"):
-            raise NotImplementedError("sampling is not part of the B200 engine (greedy / beam only)")
+            raise NotImplementedError("sampling is not part of the engine (greedy / beam only)")
         num_beams = int(generate_kwargs.get("num_beams", 1) or 1)
         if num_beams > self.max_beams:
             raise ValueError(f"num_beams={num_beams} exceeds the engine's max_beams={self.max_beams}")

@@ -1,4 +1,4 @@
-"""Streaming transcription on the B200 engine: drop-in for `thestage_speechkit.streaming.StreamingPipeline`
+"""Streaming transcription on the engine: drop-in for `thestage_speechkit.streaming.StreamingPipeline`
 (REF thestage_speechkit/streaming/streaming_pipeline.py:443-988) plus the multi-stream scheduler that replaces the
 reference's one-stream-at-a-time design (SURVEY.md §2.1 row 3, §7 step 10).
 
@@ -54,13 +54,13 @@ def words_from_result(result: Dict[str, Any], audio_duration: float, buffer_star
 
 
 class LocalWhisperBackend(TranscriptionBackend):
-    """REF :340-435 over the B200 ASRPipeline.  `platform` must be "nvidia"."""
+    """REF :340-435 over the engine's ASRPipeline.  `platform` must be "nvidia"."""
 
     def __init__(self, model, model_size: str = "S", chunk_length_s: int = 10, platform: str = "nvidia", torch_dtype=None,
                  language: str = "en", feature_extractor=None, tokenizer=None, revision: str = "main", asr_pipeline=None,
                  batch_size: int = 1, device: str = "cuda"):
         if platform != "nvidia":
-            raise ValueError(f"Invalid platform: {platform} (this build is the NVIDIA B200 engine)")
+            raise ValueError(f"Invalid platform: {platform} (this build is the NVIDIA H100 engine)")
         self.chunk_length_s = chunk_length_s
         self.sample_rate = 16000
         self.device = device

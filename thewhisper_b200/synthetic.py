@@ -27,7 +27,7 @@ PRESETS: Dict[str, dict] = {
     "large-v3": dict(d_model=1280, heads=20, ffn=5120, enc_layers=32, dec_layers=32, n_mels=128, vocab=51866),
     # whisper-large-v3-turbo: same encoder, 4 decoder layers
     "large-v3-turbo": dict(d_model=1280, heads=20, ffn=5120, enc_layers=32, dec_layers=4, n_mels=128, vocab=51866),
-    # CI-speed shapes (same id layout, same head_dim=64 so the tcgen05 attention tiles are exercised)
+    # CI-speed shapes (same id layout, same head_dim=64 so the wgmma attention tiles are exercised)
     "tiny-test": dict(d_model=128, heads=2, ffn=512, enc_layers=2, dec_layers=2, n_mels=128, vocab=51866),
     "small-test": dict(d_model=256, heads=4, ffn=1024, enc_layers=3, dec_layers=3, n_mels=128, vocab=51866),
 }

@@ -1,6 +1,6 @@
 // Microbenchmarks of the synchronisation / hand-over primitives a persistent one-CTA-per-SM decoder step is built from.
 // Every test runs a grid of one 384-thread CTA per SM through N rounds and reports ns per round (globaltimer of CTA 0).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o sync_bench sync_bench.cu && ./sync_bench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o sync_bench sync_bench.cu && ./sync_bench
 // The numbers decide which hand-over the decoder-step kernel should use (profiles/r1_v8_sync_microbench.md).
 #include <cstdio>
 #include <cstdlib>
