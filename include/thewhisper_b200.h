@@ -186,6 +186,11 @@ int bw_op_layernorm(const float* x, const float* g, const float* b, void* out, i
 /* out[M,N] fp32 = epi(LN?(x[M,K]) W[N,K]^T), M <= 8 */
 int bw_op_gemv(const float* x, const float* ln_g, const float* ln_b, const void* W, int32_t M, int32_t N, int32_t K,
                const float* bias, float alpha, int32_t act, const float* residual, float* out, void* stream);
+/* Shared-memory plan of the persistent decoder step, computed on the host (no GPU needed) by the code its launcher uses, for a
+ * device with smem_optin bytes of opt-in shared memory per block and a kernel with static_smem bytes of static shared memory:
+ * out[0] = dynamic smem bytes, out[1] = offset of the second weight-slab region (0: single-buffered slabs).  Returns 0, or -3
+ * (out[0] = 0) when the plan does not fit. */
+int bw_op_mega_plan(int32_t Q, int32_t D, int32_t ffn, int32_t num_sms, int32_t smem_optin, int32_t static_smem, int64_t* out);
 
 #ifdef __cplusplus
 }

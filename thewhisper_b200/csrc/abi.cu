@@ -147,5 +147,9 @@ int bw_op_gemv(const float* x, const float* ln_g, const float* ln_b, const void*
   g_last_f16 = 0;
   return bw_op_gemv_bf16(x, ln_g, ln_b, W, M, N, K, bias, alpha, act, residual, out, stream);
 }
+int bw_op_mega_plan(int32_t Q, int32_t D, int32_t ffn, int32_t num_sms, int32_t smem_optin, int32_t static_smem, int64_t* out) {
+  g_last_f16 = 0;
+  return bw_op_mega_plan_bf16(Q, D, ffn, num_sms, smem_optin, static_smem, out);
+}
 
 }  // extern "C"

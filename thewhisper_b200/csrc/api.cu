@@ -22,6 +22,7 @@
 #include "abi_rename.h"
 #include "../../include/thewhisper_b200.h"
 #include "decode.cuh"
+#include "decode_mega_common.cuh"
 #include "kernels.h"
 
 namespace BW_NS {
@@ -1056,6 +1057,15 @@ int bw_op_gemv(const float* x, const float* ln_g, const float* ln_b, const void*
   g.x = x; g.ldx = K; g.ln_g = ln_g; g.ln_b = ln_b; g.W = static_cast<const bf16*>(W); g.N = N; g.K = K; g.M = M;
   g.bias = bias; g.alpha = alpha; g.alpha_cols = (alpha != 1.0f) ? N : 0; g.act = act; g.residual = residual; g.out = out; g.ldo = N;
   return launch_gemv(static_cast<cudaStream_t>(stream), g);
+}
+
+int bw_op_mega_plan(int32_t Q, int32_t D, int32_t ffn, int32_t num_sms, int32_t smem_optin, int32_t static_smem, int64_t* out) {
+  BW_CHECK(out && Q >= 1 && D > 0 && ffn > 0 && num_sms > 0 && smem_optin > static_smem, "bw_op_mega_plan: bad arguments");
+  int p0_off = 0;
+  const size_t smem = mega::mega_smem_plan(Q <= 1 ? 1 : 2, D, ffn, num_sms, true, (size_t)(smem_optin - static_smem), &p0_off);
+  out[0] = (int64_t)smem;
+  out[1] = p0_off;
+  return smem ? 0 : -3;
 }
 
 }  // extern "C"

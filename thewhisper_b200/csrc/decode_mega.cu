@@ -17,7 +17,13 @@
 //     every warp), and lanes read contiguous 16-byte (x) / 8-byte (w) pieces so no LDS has bank conflicts;
 //   * 31% of the non-barrier stall samples were instruction-cache misses: the fully inlined version was 15k SASS
 //     instructions (245 KB) walked once per layer against a 32 KB L1.5 I-cache.  The six GEMV phases of a layer are
-//     therefore ONE loop body driven by a small descriptor (make_desc), not six inlined copies.
+//     therefore ONE loop body driven by a small descriptor (make_desc), not six inlined copies;
+//   * the two slab regions (double buffering, see the kernel body) must fit: the smem limit is the device's opt-in limit
+//     less the kernel's static smem as compiled.  On 132 SMs large-v3 at Q = 1 fits with 640 B to spare; an estimated
+//     8 KB margin had made every step single-buffered (H100 SXM at 700 W: 1.27 ms per step, 1.19 ms double-buffered);
+//   * more lookahead is not better: a per-CTA byte ring that requested the rows of every later phase as far ahead as
+//     ~200 KB of smem allowed, right after each barrier arrival, left no slab exposed but roughly tripled the latency of
+//     the barriers behind those ~26 MB of copies (1.41 ms per step).
 // After a barrier only the x row (and the residual values of the rows a warp owns) have to be fetched.
 //
 // Work split: 12 warps per CTA, global warp id gw; a GEMV phase gives warp gw the R rows starting at gw*R (one pass:
@@ -705,27 +711,56 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
 
 int g_mega_coop = -1;  // -1: read BW_MEGA_COOP on first use; the engine clears it if a cooperative launch cannot be captured
 
+namespace {
+
+template <int MB, unsigned VAR>
+int launch_mega(cudaStream_t st, const MegaArgs& a, int num_sms, int coop) {
+  // the shared-memory budget: the device's opt-in limit per block less this instantiation's static smem, read once
+  static size_t limit = 0, attr = 0;
+  if (!limit) {
+    int dev = 0, optin = 0;
+    BW_CUDA_OK(cudaGetDevice(&dev));
+    BW_CUDA_OK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    cudaFuncAttributes fa{};
+    BW_CUDA_OK(cudaFuncGetAttributes(&fa, decode_mega_kernel<MB, VAR>));
+    limit = (size_t)optin - fa.sharedSizeBytes;
+  }
+  MegaArgs b = a;
+  const size_t smem = mega_smem_plan(MB, a.D, a.ffn, num_sms, !(a.flags & 2), limit, &b.p0_off);
+  if (!smem) return -3;
+  if (smem > attr) {
+    BW_CUDA_OK(cudaFuncSetAttribute(decode_mega_kernel<MB, VAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 0;
+    BW_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_mega_kernel<MB, VAR>, MT, smem));
+    if (per_sm < 1) return -3;
+    attr = smem;
+  }
+  BW_CUDA_OK(cudaMemsetAsync(a.bar, 0, 1024 * sizeof(unsigned), st));
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(num_sms); cfg.blockDim = dim3(MT); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
+  cfg.attrs = at; cfg.numAttrs = coop ? 1 : 0;
+  BW_CUDA_OK(cudaLaunchKernelEx(&cfg, decode_mega_kernel<MB, VAR>, b));
+  return 0;
+}
+
+}  // namespace
+
 // Launches the persistent step kernel on `st`.  Returns -3 when the configuration is outside what it supports
 // (the caller then uses the per-op path).
 int launch_decode_mega(cudaStream_t st, const MegaArgs& a, int num_sms) {
   const int Q = a.Q;
   if (a.L > MEGA_MAXL || Q > 2 || a.D > MAXD || a.ffn > 5120 || a.D % 8 != 0 || a.ffn % 8 != 0 || a.Tmax > MAXKEYS) return -3;
   if ((size_t)MW * a.D * 2 > (size_t)ATT_OFF) return -3;  // R=1 slabs must stay below the attention scratch
-  const long long GW = (long long)num_sms * MW;
   {  // every layer GEMV is one pass of at most RMAX rows per warp
     const int nmax = 3 * a.D > a.ffn ? 3 * a.D : a.ffn;
     if (((nmax + num_sms - 1) / num_sms + MW - 1) / MW > RMAX) return -3;
   }
-  (void)GW;
   if (a.nsplit > XSPLIT) return -3;
-  const int mb = Q <= 1 ? 1 : 2;
-  MegaArgs b = a;
-  const size_t smem = mega_smem_plan(mb, a.D, a.ffn, num_sms, !(a.flags & 2), &b.p0_off);
-  if (smem + 8 * 1024 > 227 * 1024) return -3;  // the 227 KB opt-in limit includes the static smem (layer table, barriers)
   if ((size_t)((a.D + num_sms - 1) / num_sms) * a.D * 2 > (size_t)ATT_OFF) return -3;  // region-1 slabs live under the attention scratch
   const int ks = (a.S + a.nsplit - 1) / a.nsplit;
   if (ks > XKMAX) return -3;
-  BW_CUDA_OK(cudaMemsetAsync(a.bar, 0, 1024 * sizeof(unsigned), st));
   // Co-residency of the CTAs (one per SM) (round-1 advisor): the grid barriers spin, so a CTA that is not scheduled deadlocks the rest until
   // the 2^32-cycle timeout traps.  (1) the occupancy calculator must promise one CTA per SM, else -3 (per-op path); (2) the launch is
   // cooperative, so the driver either runs the whole grid at once or fails the launch (another kernel holding SMs: an error code at
@@ -735,30 +770,11 @@ int launch_decode_mega(cudaStream_t st, const MegaArgs& a, int num_sms) {
     const char* ev = getenv("BW_MEGA_COOP");
     coop = (ev && ev[0] == '0') ? 0 : 1;
   }
-#define BW_MEGA_LAUNCH(MB, VAR)                                                                                            \
-  {                                                                                                                        \
-    static size_t attr = 0;                                                                                                \
-    if (smem > attr) {                                                                                                     \
-      BW_CUDA_OK(cudaFuncSetAttribute(decode_mega_kernel<MB, VAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-      int per_sm = 0;                                                                                                      \
-      BW_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_mega_kernel<MB, VAR>, MT, smem));           \
-      if (per_sm < 1) return -3;                                                                                           \
-      attr = smem;                                                                                                         \
-    }                                                                                                                      \
-    cudaLaunchConfig_t cfg{};                                                                                              \
-    cfg.gridDim = dim3(num_sms); cfg.blockDim = dim3(MT); cfg.dynamicSmemBytes = smem; cfg.stream = st;                    \
-    cudaLaunchAttribute at[1];                                                                                             \
-    at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;                                                  \
-    cfg.attrs = at; cfg.numAttrs = coop ? 1 : 0;                                                                           \
-    BW_CUDA_OK(cudaLaunchKernelEx(&cfg, decode_mega_kernel<MB, VAR>, b));                                                  \
-  }
   // the instrumented instantiation only when a trace buffer is attached (BW_MEGA_TRACE=1)
-  if (mb == 2) {
-    if (a.trace) BW_MEGA_LAUNCH(2, 0u) else BW_MEGA_LAUNCH(2, V_NOTRACE)
-  } else {
-    if (a.trace) BW_MEGA_LAUNCH(1, 0u) else BW_MEGA_LAUNCH(1, V_NOTRACE)
-  }
-#undef BW_MEGA_LAUNCH
+  int rc;
+  if (Q <= 1) rc = a.trace ? launch_mega<1, 0u>(st, a, num_sms, coop) : launch_mega<1, V_NOTRACE>(st, a, num_sms, coop);
+  else rc = a.trace ? launch_mega<2, 0u>(st, a, num_sms, coop) : launch_mega<2, V_NOTRACE>(st, a, num_sms, coop);
+  if (rc) return rc;
   BW_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -251,8 +251,11 @@ __device__ __forceinline__ void attend_smem(const uint8_t* sK, const uint8_t* sV
   ov_out = ov;
 }
 
-// smem plan: returns the dynamic smem bytes and the offset of slab region 0 (0: single-buffered, everything at the pool's start)
-inline size_t mega_smem_plan(int mb, int D, int ffn, int num_sms, bool want_dbuf, int* p0_off) {
+// smem plan: returns the dynamic smem bytes (0: does not fit in `limit`) and the offset of slab region 0 (0: single-buffered,
+// everything at the pool's start).  limit = the device's opt-in shared memory per block less the kernel's static smem (layer
+// table, barriers): on 132 SMs the double-buffered plan for large-v3 at Q = 1 fits with a few hundred bytes to spare, so the
+// limit is taken from the device and the compiled kernel, not estimated.
+inline size_t mega_smem_plan(int mb, int D, int ffn, int num_sms, bool want_dbuf, size_t limit, int* p0_off) {
   // rows of a CTA, rounded up to whole active warps: the unused rows of the last active warp are still read (and discarded)
   auto rc = [&](int n) {
     const int rows = (n + num_sms - 1) / num_sms, R = (rows + MW - 1) / MW;
@@ -268,7 +271,6 @@ inline size_t mega_smem_plan(int mb, int D, int ffn, int num_sms, bool want_dbuf
   if (rc(ffn) * D * 2 > r0) r0 = rc(ffn) * D * 2;
   if (rc(D) * D * 2 > r0) r0 = rc(D) * D * 2;
   const size_t fixed = 64 * sizeof(float) + (size_t)mb * ffn * sizeof(float) + 128;
-  const size_t limit = 227 * 1024 - 8 * 1024;   // the opt-in limit includes the static smem (layer table, barriers)
   auto mx = [](size_t a, size_t b) { return a > b ? a : b; };
   const size_t off = (r1 + 127) / 128 * 128;
   const size_t pool_d = mx(mx(off + r0, att), lm);
@@ -277,7 +279,8 @@ inline size_t mega_smem_plan(int mb, int D, int ffn, int num_sms, bool want_dbuf
     return fixed + pool_d;
   }
   *p0_off = 0;
-  return fixed + mx(mx(mx(r0, r1), att), lm);
+  const size_t single = fixed + mx(mx(mx(r0, r1), att), lm);
+  return single <= limit ? single : 0;
 }
 
 }  // namespace mega

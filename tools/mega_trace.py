@@ -1,5 +1,5 @@
 """Barrier timeline of one persistent decoder step (BW_MEGA_TRACE=1): per phase, how long the slowest CTA worked and how
-long the barrier itself took."""
+long the barrier itself took, and per GEMV phase how long the warps waited for their weight rows after x was staged."""
 import os
 import sys
 
@@ -65,6 +65,22 @@ for ph, nm in ((0, "A qkv"), (2, "C oproj"), (3, "D xq"), (6, "G fc1"), (7, "H f
         out.append("%s %.2f/%.2f" % (lab, np.median(d), d.max()))
     out.append("arrive %.2f/%.2f" % (np.median(arr[:, i] - base) / 1e3, (arr[:, i] - base).max() / 1e3))
     print("  %-8s %s" % (nm, "  ".join(out)))
+
+# slab exposure: how long a CTA's warps waited for their weight rows after x was staged, max(0, last slab landed - x staged)
+print("slab exposure per GEMV phase, median / max over CTAs, averaged over the %d layers:" % dims.dec_layers)
+tot_med = tot_max = 0.0
+for ph, nm in ((0, "A qkv"), (2, "C oproj"), (3, "D xq"), (5, "F xo"), (6, "G fc1"), (7, "H fc2")):
+    med, mx = [], []
+    for ll in range(dims.dec_layers):
+        i = 1 + 8 * ll + ph
+        ok = mk[:, i, 0] > 0
+        e = np.maximum(0, mk[ok, i, 0] - mk[ok, i, 2]) / 1e3
+        med.append(np.median(e))
+        mx.append(e.max())
+    tot_med += np.sum(med)
+    tot_max += np.sum(mx)
+    print("  %-8s median %.2f us  max %.2f us" % (nm, np.mean(med), np.mean(mx)))
+print("  per step: sum of medians %.1f us, sum of maxima %.1f us" % (tot_med, tot_max))
 
 i = 1 + 8 * l + 4
 base = rel[:, i - 1]
