@@ -126,8 +126,8 @@ struct MegaArgs {
   float* align;
   int Ha, Tcap, step_base;
   long long* trace;  // optional barrier timeline (debug)
-  int flags;         // bit0: no L2 prefetch two phases ahead; bit1: force single-buffered weight slabs (experiments);
-                     // bit6 (64): the staging warps do not wait for the DMA warp
+  int flags;         // bit1: force single-buffered weight slabs (experiments); bit6 (64): the staging warps do not wait for
+                     // the DMA warp
   // greedy token selection fused behind the LM head (no timestamp rules, one beam): masked arg-max by 64-bit atomicMax,
   // the last CTA to finish writes the token, handles EOS / pad and advances the position -- no select kernel
   int fuse_select;

@@ -23,7 +23,16 @@
 //     8 KB margin had made every step single-buffered (H100 SXM at 700 W: 1.27 ms per step, 1.19 ms double-buffered);
 //   * more lookahead is not better: a per-CTA byte ring that requested the rows of every later phase as far ahead as
 //     ~200 KB of smem allowed, right after each barrier arrival, left no slab exposed but roughly tripled the latency of
-//     the barriers behind those ~26 MB of copies (1.41 ms per step).
+//     the barriers behind those ~26 MB of copies (1.41 ms per step);
+//   * weight rows are NOT prefetched into L2.  A DRAM -> L2 prefetch of each phase's rows two phases ahead (~13 MB for fc1
+//     and for fc2) kept the slabs from ever being exposed (0.13 us), but every barrier that ran while it was in flight slowed
+//     down: cross-q 4.0 us and cross out-proj 4.8 us instead of ~1 us (layer averages).  Keeping the prefetch W bytes ahead
+//     of the copies with a per-CTA cursor, or capping it per hand-over to even out the DRAM load, only moved that cost into
+//     other phases (1.18-1.33 ms per step for W = 8-48 MB, H100 SXM at 700 W).  With no weight prefetch the slab copy, issued a whole phase ahead
+//     into the second slab region, reads DRAM itself: the cross-q barrier falls to 1.0 us and the step from 1.19-1.20 to
+//     1.13-1.16 ms (H100 80GB HBM3, 400 W power limit).  Only the cross-attention K/V, read by a bulk load three phases
+//     later, are still prefetched: without that the cross-attention phase took 6.7 us instead of 5.9 us (the step times of the
+//     two were within each other's spread).
 // After a barrier only the x row (and the residual values of the rows a warp owns) have to be fetched.
 //
 // Work split: 12 warps per CTA, global warp id gw; a GEMV phase gives warp gw the R rows starting at gw*R (one pass:
@@ -168,14 +177,10 @@ struct Pre {
   float4 g, b;  // gamma / beta of elements [4*tid, 4*tid + 4)
 };
 
-// The rows of a CTA's 12 warps are contiguous in memory (rows [blockIdx*12*R, +12*R)) and so are their slabs in smem: one
-// TMA operation per CTA and phase.  (Per-row operations cost ~10 ns of TMA issue each -- 36 of them per SM and phase were
+// The CTA's weight rows of a layer phase: one bulk copy into a slab region, completion on that region's mbarrier.  The rows
+// of a CTA's 12 warps are contiguous in memory (rows [blockIdx*12*R, +12*R)) and so are their slabs in smem: one TMA
+// operation per CTA and phase.  (Per-row operations cost ~10 ns of TMA issue each -- 36 of them per SM and phase were
 // 0.35 us on the critical path.)
-__device__ __forceinline__ void l2_prefetch_phase(const GemvDesc& d) {
-  if (threadIdx.x == DMA_T && !d.lm && d.n0 < d.nend) l2_prefetch(d.W + (long long)d.n0 * d.K, (uint32_t)(d.nend - d.n0) * d.K * 2);
-}
-
-// The CTA's weight rows of a layer phase: one bulk copy into a slab region, completion on that region's mbarrier.
 __device__ __forceinline__ void issue_slabs(const GemvDesc& d, uint8_t* region, uint64_t* cbar) {
   if (threadIdx.x == DMA_T && d.n0 < d.nend) {
     const uint32_t bytes = (uint32_t)(d.nend - d.n0) * d.K * 2;
@@ -411,28 +416,21 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
         if (cur.residual && active && r_sel < cur.R && m < MB && m < Q && n + r_sel < cur.nend)
           res = __ldcg(cur.residual + (long long)m * cur.ldo + n + r_sel);
       }
+      // the DMA warp's turn while x is staged, when the TMA queue is empty: the slab copy of the next phase, and in the QKV
+      // phase the L2 prefetch of this layer's cross-attention K/V (DRAM -> L2, three phases before its bulk load)
       auto ahead = [&]() {
-      // two phases ahead, DRAM -> L2 (issued while the x loads of this phase are in flight, when the TMA queue is empty): a
-        // layer is ~54 MB = 8 us of HBM time spread over ~35 us, but a 13 MB slab set requested only one barrier before its
-        // use is still arriving when the phase starts, and the barrier's own atomics queue behind it
         if (dbuf && ph + 1 < nph) {
           const GemvDesc d1 = make_desc<VAR>(a, sl, (ph + 1) / 6, (ph + 1) % 6, pos);
           issue_slabs(d1, pool + (((ph + 1) & 1) ? 0 : a.p0_off), &cbar[(ph + 1) & 1]);
         }
-        if (!(a.flags & 1)) {
-          if (ph + 2 <= nph) {
-            const GemvDesc d2 = make_desc<VAR>(a, sl, ph + 2 < nph ? (ph + 2) / 6 : a.L, (ph + 2) % 6, pos);
-            l2_prefetch_phase(d2);
-          }
-          if (g == 0 && threadIdx.x == DMA_T + 1 && blockIdx.x < Q * H * nsplit) {  // this layer's cross-attention item
-            const int item = blockIdx.x;
-            const int split = item % nsplit, h = (item / nsplit) % H, q = item / (nsplit * H);
-            const int s0 = split * ks;
-            const int n = max(0, min(a.S, s0 + ks) - s0);
-            if (n > 0) {
-              l2_prefetch(L.cross_k + (((long long)q * H + h) * a.S + s0) * 64, (uint32_t)n * 128);
-              l2_prefetch(L.cross_v + (((long long)q * H + h) * a.S + s0) * 64, (uint32_t)n * 128);
-            }
+        if (g == 0 && threadIdx.x == DMA_T + 1 && blockIdx.x < Q * H * nsplit) {  // this layer's cross-attention item
+          const int item = blockIdx.x;
+          const int split = item % nsplit, h = (item / nsplit) % H, q = item / (nsplit * H);
+          const int s0 = split * ks;
+          const int n = max(0, min(a.S, s0 + ks) - s0);
+          if (n > 0) {
+            l2_prefetch(L.cross_k + (((long long)q * H + h) * a.S + s0) * 64, (uint32_t)n * 128);
+            l2_prefetch(L.cross_v + (((long long)q * H + h) * a.S + s0) * 64, (uint32_t)n * 128);
           }
         }
       };

@@ -68,7 +68,7 @@ __device__ __forceinline__ void issue_rows(uint8_t* slab, uint64_t* bar, const b
   }
 }
 
-// DRAM -> L2 only (no smem, no completion): the rows a warp will pull into its slab one phase later
+// DRAM -> L2 only (no smem, no completion): the cross-attention K/V of a layer, ahead of its bulk load
 __device__ __forceinline__ void l2_prefetch(const void* p, uint32_t bytes) {
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
 }
