@@ -96,7 +96,8 @@ int bw_encode(bw_engine* e, int32_t B, void* stream);
 /* start a decode over A audios x G sequences; prompt_host: [A*G, prompt_len] int32 */
 int bw_decode_begin(bw_engine* e, int32_t A, int32_t G, const int32_t* prompt_host, int32_t prompt_len,
                     const bw_decode_opts* opts, void* stream);
-/* run n decoder steps (one CUDA-graph launch each, no host synchronisation) */
+/* run n decoder steps (one CUDA-graph launch each, no host synchronisation).  Fails before launching anything when the
+ * steps would run past position max_target_positions - 1 (counted from bw_decode_begin) */
 int bw_decode_run(bw_engine* e, int32_t n_steps, void* stream);
 /* kernels launched by bw_decode_run since the engine was created (kernel nodes of the step graph x graph launches);
  * bench.py reports it as part of "gpu_launches" */

@@ -99,6 +99,7 @@ struct bw_engine {
   size_t align_bytes = 0;
   // current decode session
   int A = 0, G = 1, Q = 0;
+  int steps = 0;  // decoder steps run since bw_decode_begin = the device's `pos` (a step at pos = Tmax would read and write row Tmax)
   bw_decode_opts opts{};
   bool use_anc = false;
   std::map<GraphKey, cudaGraphExec_t> graphs;
@@ -796,7 +797,7 @@ int bw_decode_begin(bw_engine* e, int32_t A, int32_t G, const int32_t* prompt, i
   BW_CHECK(plen >= 1 && plen <= e->Tmax, "bw_decode_begin: prompt_len=%d out of range", plen);
   BW_CHECK(opts->begin_index >= 1 && opts->begin_index <= plen, "bw_decode_begin: begin_index=%d outside 1..prompt_len", opts->begin_index);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  e->A = A; e->G = G; e->Q = A * G; e->opts = *opts; e->use_anc = G > 1;
+  e->A = A; e->G = G; e->Q = A * G; e->opts = *opts; e->use_anc = G > 1; e->steps = 0;
   const int Q = e->Q, Tmax = e->Tmax, V = e->V;
   std::vector<int> tok((size_t)Q * Tmax, opts->pad_token);
   for (int q = 0; q < Q; ++q) memcpy(&tok[(size_t)q * Tmax], prompt + (size_t)q * plen, sizeof(int) * plen);
@@ -874,8 +875,10 @@ int bw_decode_begin(bw_engine* e, int32_t A, int32_t G, const int32_t* prompt, i
 
 int bw_decode_run(bw_engine* e, int32_t n_steps, void* stream) {
   BW_CHECK(e && e->finalized && e->Q > 0, "bw_decode_run: no decode in progress");
+  BW_CHECK(n_steps >= 0 && n_steps <= e->Tmax - e->steps, "bw_decode_run: %d steps from position %d would run past the last position %d",
+           n_steps, e->steps, e->Tmax - 1);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  for (int i = 0; i < n_steps; ++i) {
+  for (int i = 0; i < n_steps; ++i, ++e->steps) {
     if (e->cur_graph) {
       BW_CUDA_OK(cudaGraphLaunch(e->cur_graph, st));
       e->step_kernel_launches += e->graph_kernels[e->cur_graph];
