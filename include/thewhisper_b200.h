@@ -74,7 +74,11 @@ int bw_runtime_flags(void);
 int bw_engine_create(const bw_config* cfg, bw_engine** out);
 void bw_engine_destroy(bw_engine* e);
 /* Bind one weight tensor by name (device pointer, must outlive the engine).  Matrices are 16-bit (bw_config::dtype) row-major
- * [out, in] (torch Linear layout), vectors fp32.  Names: see DESIGN.md "weights". */
+ * [out, in] (torch Linear layout), vectors fp32.  Names: see DESIGN.md "weights".
+ * Int8 decoder weights (optional): "dec.embed" and every layer's "dec.<i>.wqkv", "wo", "xwq", "xwo", "w1", "w2" bound as int8
+ * codes q [out, in], each with its fp32 scale per output row s [out] bound as "<name>.scale"; the weight is s[n] * q[n, k].  The
+ * engine reads the format from the presence of "dec.embed.scale": bw_engine_finalize then requires all of those scales and
+ * otherwise rejects any.  "dec.<i>.xwk" / "xwv" (cross K/V, projected once per chunk) stay 16-bit either way. */
 int bw_engine_set_tensor(bw_engine* e, const char* name, const void* device_ptr);
 /* slaney mel filter bank [201, n_mels] fp32 on the HOST (TF/audio_utils.py:453-544), copied to the device. */
 int bw_engine_set_mel_filters(bw_engine* e, const float* bank_host);
@@ -192,6 +196,8 @@ int bw_op_gemv(const float* x, const float* ln_g, const float* ln_b, const void*
  * out[0] = dynamic smem bytes, out[1] = offset of the second weight-slab region (0: single-buffered slabs).  Returns 0, or -3
  * (out[0] = 0) when the plan does not fit. */
 int bw_op_mega_plan(int32_t Q, int32_t D, int32_t ffn, int32_t num_sms, int32_t smem_optin, int32_t static_smem, int64_t* out);
+/* The same plan for int8 decoder weights (1-byte slab rows). */
+int bw_op_mega_plan_w8(int32_t Q, int32_t D, int32_t ffn, int32_t num_sms, int32_t smem_optin, int32_t static_smem, int64_t* out);
 
 #ifdef __cplusplus
 }

@@ -75,6 +75,7 @@ SYMBOLS = {
     "bw_op_layernorm": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _P]),
     "bw_op_gemv": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _P, _F, _I, _P, _P, _P]),
     "bw_op_mega_plan": (C.c_int, [_I, _I, _I, _I, _I, _I, C.POINTER(C.c_int64)]),
+    "bw_op_mega_plan_w8": (C.c_int, [_I, _I, _I, _I, _I, _I, C.POINTER(C.c_int64)]),
 }
 
 _lib: Optional[C.CDLL] = None

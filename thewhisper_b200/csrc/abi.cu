@@ -151,5 +151,9 @@ int bw_op_mega_plan(int32_t Q, int32_t D, int32_t ffn, int32_t num_sms, int32_t 
   g_last_f16 = 0;
   return bw_op_mega_plan_bf16(Q, D, ffn, num_sms, smem_optin, static_smem, out);
 }
+int bw_op_mega_plan_w8(int32_t Q, int32_t D, int32_t ffn, int32_t num_sms, int32_t smem_optin, int32_t static_smem, int64_t* out) {
+  g_last_f16 = 0;
+  return bw_op_mega_plan_w8_bf16(Q, D, ffn, num_sms, smem_optin, static_smem, out);
+}
 
 }  // extern "C"

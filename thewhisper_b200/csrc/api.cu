@@ -48,9 +48,14 @@ struct EncLayer {
   const float *ln1g, *ln1b, *bqkv, *bo, *ln2g, *ln2b, *b1, *b2;
   const bf16 *wqkv, *wo, *w1, *w2;
 };
+// The six matrices every decoder step streams (in GEMV phase order); with int8 decoder weights they are int8 codes and
+// sc[k] is the fp32 scale per output row of kind k.  xwk / xwv (used once per chunk by the encoder) stay 16-bit.
+constexpr const char* kDecQuant[6] = {"wqkv", "wo", "xwq", "xwo", "w1", "w2"};
 struct DecLayer {
   const float *ln1g, *ln1b, *bqkv, *bo, *ln2g, *ln2b, *xbq, *xbv, *xbo, *ln3g, *ln3b, *b1, *b2;
-  const bf16 *wqkv, *wo, *xwq, *xwk, *xwv, *xwo, *w1, *w2;
+  const void *wqkv, *wo, *xwq, *xwo, *w1, *w2;
+  const bf16 *xwk, *xwv;
+  const float* sc[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
 };
 
 // Everything a captured step graph bakes in as kernel parameters: a decode that differs in any of these gets its own graph
@@ -74,7 +79,10 @@ struct bw_engine {
   bool finalized = false;
   int D, H, S, F, V, Vp, Tmax, Spad;
   // resolved weights
-  const bf16 *conv1_w = nullptr, *conv2_w = nullptr, *embed = nullptr;
+  const bf16 *conv1_w = nullptr, *conv2_w = nullptr;
+  const void* embed = nullptr;           // tied embedding / LM head: 16-bit, or int8 codes when embed_scale is bound
+  const float* embed_scale = nullptr;    // "dec.embed.scale": set iff the decoder weights are int8
+  const float** wscale_tab = nullptr;    // int8: device copy of every layer's sc[6] (the persistent step reads it)
   const float *conv1_b = nullptr, *conv2_b = nullptr, *enc_pos = nullptr, *enc_lnf_g = nullptr, *enc_lnf_b = nullptr;
   const float *dec_pos = nullptr, *dec_lnf_g = nullptr, *dec_lnf_b = nullptr;
   std::vector<EncLayer> enc;
@@ -270,15 +278,16 @@ int step_batched_impl(bw_engine* e, cudaStream_t st) {
   const long long self_layer = (long long)e->cfg.max_audios * e->cfg.max_beams * Tmax * D;
   const long long cross_layer = (long long)e->cfg.max_audios * H * S * 64;
   // raw partial sums of out[Q, N] = in[Q, K] W[N, K]^T into dpart ([split][Q][N]); returns the split count
-  auto proj = [&](const bf16* in, int K, const bf16* W, int N, int* ns) {
-    const DecGemmPlan pl = gemm_dec_plan(Q, N, K, e->num_sms, true);
+  const bool w8 = e->embed_scale != nullptr;
+  auto proj = [&](const bf16* in, int K, const void* W, const float* sc, int N, int* ns) {
+    const DecGemmPlan pl = gemm_dec_plan(Q, N, K, e->num_sms, true, w8);
     BW_CHECK((long long)pl.ksplit * N <= DPART_PER_ROW, "batched step: %d splits x N=%d exceed the partial-sum buffer", pl.ksplit, N);
     GemmEpi ep;
     ep.out_f32 = e->dpart; ep.row_stride = N;
     *ns = pl.ksplit;
-    return gemm_dec(st, in, W, Q, N, K, 0, ep, pl, (long long)Q * N);
+    return gemm_dec(st, in, W, sc, Q, N, K, 0, ep, pl, (long long)Q * N);
   };
-  if (int rc = launch_embed(st, e->embed, e->dec_pos, e->tokens, e->pos, e->dx, Q, D, Tmax)) return rc;
+  if (int rc = launch_embed(st, e->embed, e->embed_scale, e->dec_pos, e->tokens, e->pos, e->dx, Q, D, Tmax)) return rc;
   int ns = 0;                  // partial sums of the previous residual GEMM still to be folded into dx
   const float* pbias = nullptr;
   for (size_t l = 0; l < e->dec.size(); ++l) {
@@ -287,7 +296,7 @@ int step_batched_impl(bw_engine* e, cudaStream_t st) {
     bf16* vc = e->self_v + l * self_layer;
     // dx += fc2 partials of layer l-1 (+ b2); LN1 -> dbn
     if (int rc = launch_resid_ln(st, e->dx, e->dpart, ns, (long long)Q * D, pbias, L.ln1g, L.ln1b, e->dbn, Q, D)) return rc;
-    if (int rc = proj(e->dbn, D, L.wqkv, 3 * D, &ns)) return rc;
+    if (int rc = proj(e->dbn, D, L.wqkv, L.sc[0], 3 * D, &ns)) return rc;
     {
       SelfAttnArgs s;
       s.qkv = e->dpart; s.nsplit = ns; s.split_stride = (long long)Q * 3 * D; s.qkv_bias = L.bqkv; s.q_alpha = 0.125f;
@@ -295,9 +304,9 @@ int step_batched_impl(bw_engine* e, cudaStream_t st) {
       s.H = H; s.D = D; s.Tmax = Tmax;
       if (int rc = launch_self_attn(st, s, Q)) return rc;
     }
-    if (int rc = proj(e->dba, D, L.wo, D, &ns)) return rc;
+    if (int rc = proj(e->dba, D, L.wo, L.sc[1], D, &ns)) return rc;
     if (int rc = launch_resid_ln(st, e->dx, e->dpart, ns, (long long)Q * D, L.bo, L.ln2g, L.ln2b, e->dbn, Q, D)) return rc;
-    if (int rc = proj(e->dbn, D, L.xwq, D, &ns)) return rc;
+    if (int rc = proj(e->dbn, D, L.xwq, L.sc[2], D, &ns)) return rc;
     {
       CrossAttnArgs c;
       c.q = e->dpart; c.nsplit = ns; c.split_stride = (long long)Q * D; c.q_bias = L.xbq; c.q_alpha = 0.125f;
@@ -310,19 +319,19 @@ int step_batched_impl(bw_engine* e, cudaStream_t st) {
       }
       if (int rc = launch_cross_attn(st, c, A)) return rc;
     }
-    if (int rc = proj(e->dba, D, L.xwo, D, &ns)) return rc;
+    if (int rc = proj(e->dba, D, L.xwo, L.sc[3], D, &ns)) return rc;
     if (int rc = launch_resid_ln(st, e->dx, e->dpart, ns, (long long)Q * D, L.xbo, L.ln3g, L.ln3b, e->dbn, Q, D)) return rc;
-    if (int rc = proj(e->dbn, D, L.w1, ffn, &ns)) return rc;
+    if (int rc = proj(e->dbn, D, L.w1, L.sc[4], ffn, &ns)) return rc;
     if (int rc = launch_gelu_bias(st, e->dpart, ns, (long long)Q * ffn, L.b1, e->dbh, Q, ffn)) return rc;
-    if (int rc = proj(e->dbh, ffn, L.w2, D, &ns)) return rc;
+    if (int rc = proj(e->dbh, ffn, L.w2, L.sc[5], D, &ns)) return rc;
     pbias = L.b2;
   }
   if (int rc = launch_resid_ln(st, e->dx, e->dpart, ns, (long long)Q * D, pbias, e->dec_lnf_g, e->dec_lnf_b, e->dbn, Q, D)) return rc;
   {  // tied LM head: 406 weight tiles, no split; rows of the embedding beyond V are zero-filled by TMA and not stored
-    const DecGemmPlan pl = gemm_dec_plan(Q, e->V, D, e->num_sms, false);
+    const DecGemmPlan pl = gemm_dec_plan(Q, e->V, D, e->num_sms, false, w8);
     GemmEpi ep;
     ep.out_f32 = e->logits; ep.row_stride = e->Vp;
-    if (int rc = gemm_dec(st, e->dbn, e->embed, Q, e->V, D, e->V, ep, pl, 0)) return rc;
+    if (int rc = gemm_dec(st, e->dbn, e->embed, e->embed_scale, Q, e->V, D, e->V, ep, pl, 0)) return rc;
   }
   return 0;
 }
@@ -347,7 +356,7 @@ int step_impl(bw_engine* e, cudaStream_t st) {
       o.head_slots = (e->opts.record_alignment && e->cfg.n_align_heads > 0) ? e->head_slots + l * H : nullptr;
     }
     m.L = (int)e->dec.size(); m.D = D; m.H = H; m.ffn = ffn; m.V = V; m.S = S; m.Tmax = Tmax; m.Q = Q;
-    m.embed = e->embed; m.dec_pos = e->dec_pos; m.lnf_g = e->dec_lnf_g; m.lnf_b = e->dec_lnf_b;
+    m.embed = e->embed; m.embed_scale = e->embed_scale; m.wscale = e->wscale_tab; m.dec_pos = e->dec_pos; m.lnf_g = e->dec_lnf_g; m.lnf_b = e->dec_lnf_b;
     m.tokens = e->tokens; m.pos = e->pos; m.ldl = e->Vp;
     m.dx = e->dx; m.dqkv = e->dqkv; m.dattn = e->dattn; m.dq = e->dq; m.dh = e->dh; m.logits = e->logits;
     m.part_o = e->part_o; m.part_ml = e->part_ml; m.xcounters = e->xcounters; m.bar = e->mega_bar;
@@ -379,7 +388,7 @@ int step_impl(bw_engine* e, cudaStream_t st) {
     mega_done = true;
   }
   if (!mega_done) {
-  if (int rc = launch_embed(st, e->embed, e->dec_pos, e->tokens, e->pos, e->dx, Q, D, Tmax)) return rc;
+  if (int rc = launch_embed(st, e->embed, e->embed_scale, e->dec_pos, e->tokens, e->pos, e->dx, Q, D, Tmax)) return rc;
   const long long self_layer = (long long)e->cfg.max_audios * e->cfg.max_beams * Tmax * D;
   const long long cross_layer = (long long)e->cfg.max_audios * H * S * 64;
   for (size_t l = 0; l < e->dec.size(); ++l) {
@@ -391,7 +400,7 @@ int step_impl(bw_engine* e, cudaStream_t st) {
       GemvArgs g;
       g.M = Q - m0;
       g.x = e->dx + (long long)m0 * D; g.ldx = D; g.ln_g = L.ln1g; g.ln_b = L.ln1b;
-      g.W = L.wqkv; g.N = 3 * D; g.K = D; g.bias = L.bqkv; g.alpha = 0.125f; g.alpha_cols = D;
+      g.W = L.wqkv; g.wscale = L.sc[0]; g.N = 3 * D; g.K = D; g.bias = L.bqkv; g.alpha = 0.125f; g.alpha_cols = D;
       g.out = e->dqkv + (long long)m0 * 3 * D; g.ldo = 3 * D;
       g.kc = kc; g.vc = vc; g.D = D; g.Tmax = Tmax; g.seq0 = m0; g.pos = e->pos;
       if (int rc = launch_gemv(st, g)) return rc;
@@ -406,7 +415,7 @@ int step_impl(bw_engine* e, cudaStream_t st) {
        // out-proj + residual
       GemvArgs g;
       g.M = Q - m0;
-      g.x = e->dattn + (long long)m0 * D; g.ldx = D; g.W = L.wo; g.N = D; g.K = D; g.bias = L.bo;
+      g.x = e->dattn + (long long)m0 * D; g.ldx = D; g.W = L.wo; g.wscale = L.sc[1]; g.N = D; g.K = D; g.bias = L.bo;
       g.residual = e->dx + (long long)m0 * D; g.out = e->dx + (long long)m0 * D; g.ldo = D;
       if (int rc = launch_gemv(st, g)) return rc;
     }
@@ -415,7 +424,7 @@ int step_impl(bw_engine* e, cudaStream_t st) {
       GemvArgs g;
       g.M = Q - m0;
       g.x = e->dx + (long long)m0 * D; g.ldx = D; g.ln_g = L.ln2g; g.ln_b = L.ln2b;
-      g.W = L.xwq; g.N = D; g.K = D; g.bias = L.xbq; g.alpha = 0.125f; g.alpha_cols = D;
+      g.W = L.xwq; g.wscale = L.sc[2]; g.N = D; g.K = D; g.bias = L.xbq; g.alpha = 0.125f; g.alpha_cols = D;
       g.out = e->dq + (long long)m0 * D; g.ldo = D;
       if (int rc = launch_gemv(st, g)) return rc;
     }
@@ -434,7 +443,7 @@ int step_impl(bw_engine* e, cudaStream_t st) {
        // cross out-proj + residual
       GemvArgs g;
       g.M = Q - m0;
-      g.x = e->dattn + (long long)m0 * D; g.ldx = D; g.W = L.xwo; g.N = D; g.K = D; g.bias = L.xbo;
+      g.x = e->dattn + (long long)m0 * D; g.ldx = D; g.W = L.xwo; g.wscale = L.sc[3]; g.N = D; g.K = D; g.bias = L.xbo;
       g.residual = e->dx + (long long)m0 * D; g.out = e->dx + (long long)m0 * D; g.ldo = D;
       if (int rc = launch_gemv(st, g)) return rc;
     }
@@ -443,7 +452,7 @@ int step_impl(bw_engine* e, cudaStream_t st) {
       GemvArgs g;
       g.M = Q - m0;
       g.x = e->dx + (long long)m0 * D; g.ldx = D; g.ln_g = L.ln3g; g.ln_b = L.ln3b;
-      g.W = L.w1; g.N = ffn; g.K = D; g.bias = L.b1; g.act = 1;
+      g.W = L.w1; g.wscale = L.sc[4]; g.N = ffn; g.K = D; g.bias = L.b1; g.act = 1;
       g.out = e->dh + (long long)m0 * ffn; g.ldo = ffn;
       if (int rc = launch_gemv(st, g)) return rc;
     }
@@ -451,7 +460,7 @@ int step_impl(bw_engine* e, cudaStream_t st) {
        // fc2 + residual
       GemvArgs g;
       g.M = Q - m0;
-      g.x = e->dh + (long long)m0 * ffn; g.ldx = ffn; g.W = L.w2; g.N = D; g.K = ffn; g.bias = L.b2;
+      g.x = e->dh + (long long)m0 * ffn; g.ldx = ffn; g.W = L.w2; g.wscale = L.sc[5]; g.N = D; g.K = ffn; g.bias = L.b2;
       g.residual = e->dx + (long long)m0 * D; g.out = e->dx + (long long)m0 * D; g.ldo = D;
       if (int rc = launch_gemv(st, g)) return rc;
     }
@@ -461,7 +470,7 @@ int step_impl(bw_engine* e, cudaStream_t st) {
     GemvArgs g;
     g.M = Q - m0;
     g.x = e->dx + (long long)m0 * D; g.ldx = D; g.ln_g = e->dec_lnf_g; g.ln_b = e->dec_lnf_b;
-    g.W = e->embed; g.N = V; g.K = D;
+    g.W = e->embed; g.wscale = e->embed_scale; g.N = V; g.K = D;
     g.out = e->logits + (long long)m0 * e->Vp; g.ldo = e->Vp;
     if (int rc = launch_gemv(st, g)) return rc;
   }
@@ -614,7 +623,7 @@ int bw_engine_finalize(bw_engine* e) {
   NEED(bf16, e->conv1_w, "enc.conv1.w") NEED(float, e->conv1_b, "enc.conv1.b")
   NEED(bf16, e->conv2_w, "enc.conv2.w") NEED(float, e->conv2_b, "enc.conv2.b")
   NEED(float, e->enc_pos, "enc.pos") NEED(float, e->enc_lnf_g, "enc.lnf.g") NEED(float, e->enc_lnf_b, "enc.lnf.b")
-  NEED(bf16, e->embed, "dec.embed") NEED(float, e->dec_pos, "dec.pos")
+  NEED(void, e->embed, "dec.embed") NEED(float, e->dec_pos, "dec.pos")
   NEED(float, e->dec_lnf_g, "dec.lnf.g") NEED(float, e->dec_lnf_b, "dec.lnf.b")
   e->enc.resize(c.enc_layers);
   for (int i = 0; i < c.enc_layers; ++i) {
@@ -628,12 +637,41 @@ int bw_engine_finalize(bw_engine* e) {
   for (int i = 0; i < c.dec_layers; ++i) {
     const std::string p = "dec." + std::to_string(i) + ".";
     DecLayer& L = e->dec[i];
-    NEED(float, L.ln1g, p + "ln1.g") NEED(float, L.ln1b, p + "ln1.b") NEED(bf16, L.wqkv, p + "wqkv") NEED(float, L.bqkv, p + "bqkv")
-    NEED(bf16, L.wo, p + "wo") NEED(float, L.bo, p + "bo") NEED(float, L.ln2g, p + "ln2.g") NEED(float, L.ln2b, p + "ln2.b")
-    NEED(bf16, L.xwq, p + "xwq") NEED(float, L.xbq, p + "xbq") NEED(bf16, L.xwk, p + "xwk") NEED(bf16, L.xwv, p + "xwv")
-    NEED(float, L.xbv, p + "xbv") NEED(bf16, L.xwo, p + "xwo") NEED(float, L.xbo, p + "xbo")
+    NEED(float, L.ln1g, p + "ln1.g") NEED(float, L.ln1b, p + "ln1.b") NEED(void, L.wqkv, p + "wqkv") NEED(float, L.bqkv, p + "bqkv")
+    NEED(void, L.wo, p + "wo") NEED(float, L.bo, p + "bo") NEED(float, L.ln2g, p + "ln2.g") NEED(float, L.ln2b, p + "ln2.b")
+    NEED(void, L.xwq, p + "xwq") NEED(float, L.xbq, p + "xbq") NEED(bf16, L.xwk, p + "xwk") NEED(bf16, L.xwv, p + "xwv")
+    NEED(float, L.xbv, p + "xbv") NEED(void, L.xwo, p + "xwo") NEED(float, L.xbo, p + "xbo")
     NEED(float, L.ln3g, p + "ln3.g") NEED(float, L.ln3b, p + "ln3.b")
-    NEED(bf16, L.w1, p + "w1") NEED(float, L.b1, p + "b1") NEED(bf16, L.w2, p + "w2") NEED(float, L.b2, p + "b2")
+    NEED(void, L.w1, p + "w1") NEED(float, L.b1, p + "b1") NEED(void, L.w2, p + "w2") NEED(float, L.b2, p + "b2")
+  }
+  {  // int8 decoder weights: "dec.embed.scale" bound -> every layer binds the scales of all six kinds; otherwise no scale at all
+    const bool w8 = e->tensors.count("dec.embed.scale") != 0;
+    std::map<std::string, bool> want;
+    if (w8) NEED(float, e->embed_scale, "dec.embed.scale")
+    want["dec.embed.scale"] = true;
+    for (int i = 0; i < c.dec_layers; ++i) {
+      for (int k = 0; k < 6; ++k) {
+        const std::string n = "dec." + std::to_string(i) + "." + kDecQuant[k] + ".scale";
+        want[n] = true;
+        if (w8) {
+          BW_CHECK(e->tensors.count(n), "int8 decoder weights: scale '%s' is not bound ('dec.embed.scale' is)", n.c_str());
+          NEED(float, e->dec[i].sc[k], n)
+        }
+      }
+    }
+    for (const auto& kv : e->tensors) {
+      const std::string& n = kv.first;
+      if (n.size() > 6 && n.compare(n.size() - 6, 6, ".scale") == 0) {
+        BW_CHECK(want.count(n), "weight '%s': only the int8 decoder matrices (dec.embed, dec.<i>.{wqkv,wo,xwq,xwo,w1,w2}) have scales", n.c_str());
+        BW_CHECK(w8, "scale '%s' is bound but 'dec.embed.scale' is not: int8 decoder weights need the scales of all seven kinds", n.c_str());
+      }
+    }
+    if (w8) {
+      std::vector<const float*> tab;
+      for (const DecLayer& L : e->dec) tab.insert(tab.end(), L.sc, L.sc + 6);
+      if (dalloc(e, "wscale_tab", &e->wscale_tab, tab.size())) return -1;
+      BW_CUDA_OK(cudaMemcpy(e->wscale_tab, tab.data(), tab.size() * sizeof(const float*), cudaMemcpyHostToDevice));
+    }
   }
 #undef NEED
   BW_CHECK(e->mel_plan != nullptr, "mel filter bank not set (bw_engine_set_mel_filters)");
@@ -1021,7 +1059,7 @@ int bw_op_gemm_dec(const void* X, const void* W, int32_t Q, int32_t N, int32_t K
   *ksplit_used = pl.ksplit;
   GemmEpi ep;
   ep.out_f32 = out_partials; ep.row_stride = N;
-  return gemm_dec(static_cast<cudaStream_t>(stream), static_cast<const bf16*>(X), static_cast<const bf16*>(W), Q, N, K, n_valid, ep, pl, (long long)Q * N);
+  return gemm_dec(static_cast<cudaStream_t>(stream), static_cast<const bf16*>(X), W, nullptr, Q, N, K, n_valid, ep, pl, (long long)Q * N);
 }
 
 int bw_op_gelu_bias(const float* partials, int32_t nsplit, const float* bias, void* h_bf16, int32_t Q, int32_t N, void* stream) {
@@ -1062,13 +1100,21 @@ int bw_op_gemv(const float* x, const float* ln_g, const float* ln_b, const void*
   return launch_gemv(static_cast<cudaStream_t>(stream), g);
 }
 
-int bw_op_mega_plan(int32_t Q, int32_t D, int32_t ffn, int32_t num_sms, int32_t smem_optin, int32_t static_smem, int64_t* out) {
+static int mega_plan(int32_t Q, int32_t D, int32_t ffn, int32_t num_sms, int32_t smem_optin, int32_t static_smem, int64_t* out, int esz) {
   BW_CHECK(out && Q >= 1 && D > 0 && ffn > 0 && num_sms > 0 && smem_optin > static_smem, "bw_op_mega_plan: bad arguments");
   int p0_off = 0;
-  const size_t smem = mega::mega_smem_plan(Q <= 1 ? 1 : 2, D, ffn, num_sms, true, (size_t)(smem_optin - static_smem), &p0_off);
+  const size_t smem = mega::mega_smem_plan(Q <= 1 ? 1 : 2, D, ffn, num_sms, true, (size_t)(smem_optin - static_smem), &p0_off, esz);
   out[0] = (int64_t)smem;
   out[1] = p0_off;
   return smem ? 0 : -3;
+}
+
+int bw_op_mega_plan(int32_t Q, int32_t D, int32_t ffn, int32_t num_sms, int32_t smem_optin, int32_t static_smem, int64_t* out) {
+  return mega_plan(Q, D, ffn, num_sms, smem_optin, static_smem, out, 2);
+}
+
+int bw_op_mega_plan_w8(int32_t Q, int32_t D, int32_t ffn, int32_t num_sms, int32_t smem_optin, int32_t static_smem, int64_t* out) {
+  return mega_plan(Q, D, ffn, num_sms, smem_optin, static_smem, out, 1);
 }
 
 }  // extern "C"

@@ -103,6 +103,17 @@ __device__ __forceinline__ float2 unpack_bf16(uint32_t u) {
 }
 #endif
 
+// Four signed int8 weight codes (int8 decoder weights) -> four exact floats without I2F (16 per clock per SM on sm_90): byte
+// b + 128 is permuted into the low mantissa byte of 2^23 (0x4B0000xx = 2^23 + b + 128), one FADD removes 2^23 + 128.
+// A zero word gives four zeros.
+__device__ __forceinline__ void unpack_s8x4(uint32_t u, float (&f)[4]) {
+  const uint32_t b = u ^ 0x80808080u;
+  f[0] = __uint_as_float(__byte_perm(b, 0x4B000000u, 0x7540)) - 8388736.f;
+  f[1] = __uint_as_float(__byte_perm(b, 0x4B000000u, 0x7541)) - 8388736.f;
+  f[2] = __uint_as_float(__byte_perm(b, 0x4B000000u, 0x7542)) - 8388736.f;
+  f[3] = __uint_as_float(__byte_perm(b, 0x4B000000u, 0x7543)) - 8388736.f;
+}
+
 // 16-byte streaming load that does not pollute L1 (weights / KV are read once per step)
 __device__ __forceinline__ uint4 ld_nc_u4(const void* p) {
   uint4 r;
@@ -112,6 +123,11 @@ __device__ __forceinline__ uint4 ld_nc_u4(const void* p) {
                : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
                : "l"(p)
                : "memory");
+  return r;
+}
+__device__ __forceinline__ uint2 ld_nc_u2(const void* p) {
+  uint2 r;
+  asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p) : "memory");
   return r;
 }
 
@@ -329,6 +345,9 @@ __device__ __forceinline__ void wg_kblock(float (&d)[BN / 2], uint32_t sa, uint3
 // for the 128-byte swizzle used everywhere here).
 int make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t row_pitch_bytes,
                       uint32_t box_rows, uint32_t box_cols);
+// the same for a 2-D uint8 tensor (int8 weight codes), unswizzled: box_cols bytes per row
+int make_tmap_2d_u8(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t row_pitch_bytes, uint32_t box_rows,
+                    uint32_t box_cols);
 // multiprocessor count of the current device (queried once)
 int device_sms();
 

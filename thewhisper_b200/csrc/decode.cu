@@ -25,6 +25,18 @@ __global__ void embed_kernel(const bf16* __restrict__ E, const float* __restrict
   for (int d = threadIdx.x; d < D; d += blockDim.x)
     x[(long long)q * D + d] = e2f(E[(long long)tok * D + d]) + P[(long long)pos * D + d];
 }
+// int8 embedding: x[q, :] = Es[t] * E[t, :] + P[pos, :], t = token[q, pos]
+__global__ void embed_s8_kernel(const int8_t* __restrict__ E, const float* __restrict__ Es, const float* __restrict__ P,
+                                const int* __restrict__ tokens, const int* __restrict__ pos_ptr, float* __restrict__ x, int D, int Tmax) {
+  const int q = blockIdx.x;
+  pdl_wait();
+  pdl_launch();
+  const int pos = *pos_ptr;
+  const int tok = tokens[q * Tmax + pos];
+  const float s = Es[tok];
+  for (int d = threadIdx.x; d < D; d += blockDim.x)
+    x[(long long)q * D + d] = s * (float)E[(long long)tok * D + d] + P[(long long)pos * D + d];
+}
 
 // ------------------------------------------------------------------------------------------------
 // token selection: suppress masks + Whisper timestamp rules + greedy argmax, one block per sequence
@@ -344,8 +356,10 @@ int launch_resid_ln(cudaStream_t st, float* x, const float* part, int nsplit, lo
   return 0;
 }
 
-int launch_embed(cudaStream_t st, const bf16* E, const float* P, const int* tokens, const int* pos, float* x, int Q, int D, int Tmax) {
-  BW_CUDA_OK(launch_k(embed_kernel, dim3(Q), dim3(256), 0, st, E, P, tokens, pos, x, D, Tmax));
+int launch_embed(cudaStream_t st, const void* E, const float* Es, const float* P, const int* tokens, const int* pos, float* x, int Q, int D,
+                 int Tmax) {
+  if (Es) BW_CUDA_OK(launch_k(embed_s8_kernel, dim3(Q), dim3(256), 0, st, static_cast<const int8_t*>(E), Es, P, tokens, pos, x, D, Tmax));
+  else BW_CUDA_OK(launch_k(embed_kernel, dim3(Q), dim3(256), 0, st, static_cast<const bf16*>(E), P, tokens, pos, x, D, Tmax));
   return 0;
 }
 

@@ -10,7 +10,8 @@ struct GemvArgs {
   int ldx = 0;
   const float* ln_g = nullptr;  // optional LayerNorm (eps 1e-5) applied to x rows first
   const float* ln_b = nullptr;
-  const bf16* W = nullptr;  // [N, K]
+  const void* W = nullptr;  // [N, K] 16-bit, or int8 codes when wscale is set
+  const float* wscale = nullptr;  // int8 weights: fp32 scale per row n, applied to the dot product before the bias
   int N = 0, K = 0, M = 0;
   const float* bias = nullptr;
   float alpha = 1.0f;
@@ -96,7 +97,7 @@ struct SelectArgs {
 // ---- persistent one-kernel-per-step decoder (decode_mega.cu) ----
 struct MegaLayer {
   const float *ln1g, *ln1b, *bqkv, *bo, *ln2g, *ln2b, *xbq, *xbo, *ln3g, *ln3b, *b1, *b2;
-  const bf16 *wqkv, *wo, *xwq, *xwo, *w1, *w2;
+  const void *wqkv, *wo, *xwq, *xwo, *w1, *w2;  // 16-bit, or int8 codes when MegaArgs::embed_scale is set
   bf16 *self_k, *self_v;
   const bf16 *cross_k, *cross_v;
   const int* head_slots;  // [H] or null
@@ -112,7 +113,7 @@ struct MegaArgs {
   MegaLayer layers[MEGA_MAXL];
   int L, D, H, ffn, V, S, Tmax, Q;
   int ldl;  // row pitch of logits (V rounded up to 32: rows stay 16-byte aligned for the batched path's wgmma LM head)
-  const bf16* embed;
+  const void* embed;
   const float* dec_pos;
   const float *lnf_g, *lnf_b;
   const int* tokens;
@@ -140,13 +141,19 @@ struct MegaArgs {
   unsigned long long* sel_best;  // [Q], zero between steps
   unsigned* sel_ctr;             // zero between steps
   int p0_off;        // set by the launcher: byte offset of the second slab region (0: single-buffered slabs)
+  // int8 decoder weights (set iff embed_scale is): a device table [L][6] of the row-scale pointers of wqkv, wo, xwq, xwo, w1, w2
+  // (GEMV phase order), and the scales of the tied embedding.  Neither in the smem layer table (the static smem does not grow)
+  // nor as 1.5 KB of per-layer pointers in the parameter block the 16-bit step launches with too.
+  const float* const* wscale;
+  const float* embed_scale;
 };
 
 // Returns -3 when the configuration is outside what the persistent kernel supports (caller uses the per-op path).
 int launch_decode_mega(cudaStream_t st, const MegaArgs& a, int num_sms);
 extern int g_mega_coop;  // 1: the persistent step kernels are launched cooperatively (co-residency guaranteed by the driver)
 int launch_gemv(cudaStream_t st, const GemvArgs& a);
-int launch_embed(cudaStream_t st, const bf16* E, const float* P, const int* tokens, const int* pos, float* x, int Q, int D, int Tmax);
+// E: 16-bit rows, or int8 codes with per-row scales Es (x = Es[t] * E[t] + P[pos])
+int launch_embed(cudaStream_t st, const void* E, const float* Es, const float* P, const int* tokens, const int* pos, float* x, int Q, int D, int Tmax);
 int launch_self_attn(cudaStream_t st, const SelfAttnArgs& a, int Q);
 int launch_cross_attn(cudaStream_t st, const CrossAttnArgs& a, int A);
 int launch_select(cudaStream_t st, const SelectArgs& a);

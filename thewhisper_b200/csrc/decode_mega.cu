@@ -106,7 +106,8 @@ struct GridBar {
 
 // One GEMV phase: out[m][n] = epi(sum_k W[n][k] * LN?(src[m])[k] + bias[n]).
 struct GemvDesc {
-  const bf16* W;
+  const uint8_t* W;       // rows of K elements: 16-bit, or int8 codes (W8 instantiation)
+  const float* scale;     // W8: fp32 scale per row, applied to the finished dot product before the bias
   const float* bias;
   int N, K, R;            // R rows per warp (1 .. RMAX)
   int n0, nend;           // rows of this CTA: [n0, nend), contiguous, ceil(N / CTAs) each (the LM head streams: [0, N))
@@ -129,9 +130,11 @@ __device__ __forceinline__ void split_rows(GemvDesc& d) {
   d.n0 = min(d.N, (int)blockIdx.x * rc);
   d.nend = min(d.N, d.n0 + rc);
 }
-template <unsigned VAR>
+template <unsigned VAR, bool W8>
 __device__ __forceinline__ GemvDesc make_desc(const MegaArgs& a, const MegaLayer* layers, int l, int g, int pos) {
   GemvDesc d;
+  d.scale = nullptr;
+  if constexpr (W8) d.scale = l >= a.L ? a.embed_scale : a.wscale[l * 6 + g];
   d.lng = d.lnb = nullptr;
   d.residual = nullptr;
   d.act = 0;
@@ -141,29 +144,29 @@ __device__ __forceinline__ GemvDesc make_desc(const MegaArgs& a, const MegaLayer
   d.N = d.K = d.ldo = a.D;
   d.lm = false;
   if (l >= a.L) {
-    d.W = a.embed; d.bias = nullptr; d.N = a.V; d.R = 2; d.n0 = 0; d.nend = a.V; d.lm = true; d.src = a.dx; d.lng = a.lnf_g; d.lnb = a.lnf_b; d.out = a.logits; d.ldo = a.ldl;
+    d.W = static_cast<const uint8_t*>(a.embed); d.bias = nullptr; d.N = a.V; d.R = 2; d.n0 = 0; d.nend = a.V; d.lm = true; d.src = a.dx; d.lng = a.lnf_g; d.lnb = a.lnf_b; d.out = a.logits; d.ldo = a.ldl;
     return d;
   }
   const MegaLayer& L = layers[l];
   switch (g) {
     case 0:
-      d.W = L.wqkv; d.bias = L.bqkv; d.N = 3 * a.D; d.src = a.dx; d.lng = L.ln1g; d.lnb = L.ln1b; d.out = a.dqkv; d.ldo = 3 * a.D;
+      d.W = static_cast<const uint8_t*>(L.wqkv); d.bias = L.bqkv; d.N = 3 * a.D; d.src = a.dx; d.lng = L.ln1g; d.lnb = L.ln1b; d.out = a.dqkv; d.ldo = 3 * a.D;
       d.alpha = 0.125f; d.alpha_cols = a.D; d.kc = L.self_k; d.vc = L.self_v;
       break;
     case 1:
-      d.W = L.wo; d.bias = L.bo; d.src = a.dattn; d.out = a.dx; d.residual = a.dx;
+      d.W = static_cast<const uint8_t*>(L.wo); d.bias = L.bo; d.src = a.dattn; d.out = a.dx; d.residual = a.dx;
       break;
     case 2:
-      d.W = L.xwq; d.bias = L.xbq; d.src = a.dx; d.lng = L.ln2g; d.lnb = L.ln2b; d.out = a.dq; d.alpha = 0.125f; d.alpha_cols = a.D;
+      d.W = static_cast<const uint8_t*>(L.xwq); d.bias = L.xbq; d.src = a.dx; d.lng = L.ln2g; d.lnb = L.ln2b; d.out = a.dq; d.alpha = 0.125f; d.alpha_cols = a.D;
       break;
     case 3:
-      d.W = L.xwo; d.bias = L.xbo; d.src = a.dattn; d.out = a.dx; d.residual = a.dx;
+      d.W = static_cast<const uint8_t*>(L.xwo); d.bias = L.xbo; d.src = a.dattn; d.out = a.dx; d.residual = a.dx;
       break;
     case 4:
-      d.W = L.w1; d.bias = L.b1; d.N = a.ffn; d.src = a.dx; d.lng = L.ln3g; d.lnb = L.ln3b; d.out = a.dh; d.ldo = a.ffn; d.act = 1;
+      d.W = static_cast<const uint8_t*>(L.w1); d.bias = L.b1; d.N = a.ffn; d.src = a.dx; d.lng = L.ln3g; d.lnb = L.ln3b; d.out = a.dh; d.ldo = a.ffn; d.act = 1;
       break;
     default:
-      d.W = L.w2; d.bias = L.b2; d.K = a.ffn; d.src = a.dh; d.out = a.dx; d.residual = a.dx;
+      d.W = static_cast<const uint8_t*>(L.w2); d.bias = L.b2; d.K = a.ffn; d.src = a.dh; d.out = a.dx; d.residual = a.dx;
       break;
   }
   split_rows(d);
@@ -174,6 +177,7 @@ __device__ __forceinline__ GemvDesc make_desc(const MegaArgs& a, const MegaLayer
 // row into the warp's slab, completion on the warp's mbarrier), the bias values and this thread's LayerNorm slice.
 struct Pre {
   float bias;   // of the row this lane finishes (lanes [8r, 8r + MB) finish row n + r)
+  float scale;  // W8: the scale of that row
   float4 g, b;  // gamma / beta of elements [4*tid, 4*tid + 4)
 };
 
@@ -181,27 +185,32 @@ struct Pre {
 // of a CTA's 12 warps are contiguous in memory (rows [blockIdx*12*R, +12*R)) and so are their slabs in smem: one TMA
 // operation per CTA and phase.  (Per-row operations cost ~10 ns of TMA issue each -- 36 of them per SM and phase were
 // 0.35 us on the critical path.)
+template <int ESZ>
 __device__ __forceinline__ void issue_slabs(const GemvDesc& d, uint8_t* region, uint64_t* cbar) {
   if (threadIdx.x == DMA_T && d.n0 < d.nend) {
-    const uint32_t bytes = (uint32_t)(d.nend - d.n0) * d.K * 2;
+    const uint32_t bytes = (uint32_t)(d.nend - d.n0) * d.K * ESZ;
     mbar_arrive_expect_tx(cbar, bytes);
-    bulk_g2s(region, d.W + (long long)d.n0 * d.K, bytes, cbar);
+    if constexpr (ESZ == 2) bulk_g2s(region, reinterpret_cast<const bf16*>(d.W) + (long long)d.n0 * d.K, bytes, cbar);
+    else bulk_g2s(region, d.W + (long long)d.n0 * d.K, bytes, cbar);
   }
 }
 
 // What is requested before the barrier that precedes a GEMV phase (besides the slabs): the bias of the row a lane will
 // finish and this thread's LayerNorm slice.  The LM head (many passes) uses per-warp slabs and barriers: its passes are
 // refilled warp by warp; its first pass is requested here.
+template <bool W8>
 __device__ __forceinline__ void prefetch_phase(const GemvDesc& d, Pre& p, uint8_t* pool, uint64_t* wbar, int gw, int warp, int lane) {
+  constexpr int ESZ = W8 ? 1 : 2;
   int n;
   if (d.lm) {
     n = gw * d.R;
-    if (n < d.N) issue_rows(pool + (size_t)warp * d.R * d.K * 2, wbar, d.W, d.K, d.R, n, d.N, lane);
+    if (n < d.N) issue_rows<ESZ>(pool + (size_t)warp * d.R * d.K * ESZ, wbar, d.W, d.K, d.R, n, d.N, lane);
   } else {
     n = d.n0 + warp * d.R;
   }
   const int r_sel = lane >> 3;
   p.bias = (d.bias && (lane & 7) < 2 && r_sel < d.R && n + r_sel < d.nend) ? d.bias[n + r_sel] : 0.f;
+  if constexpr (W8) p.scale = (!d.lm && (lane & 7) < 2 && r_sel < d.R && n + r_sel < d.nend) ? d.scale[n + r_sel] : 1.f;
   const int k = threadIdx.x * 4;
   if (d.lng && k < d.K) {
     p.g = *reinterpret_cast<const float4*>(d.lng + k);
@@ -305,10 +314,10 @@ __device__ __forceinline__ void stage_x(float* xs, float* red, const GemvDesc& d
   else __syncthreads();
 }
 
-// lanes [8r, 8r + MB) finish row n + r  (R <= RMAX = 4, MB <= 8)
-template <int MB, unsigned VAR>
-__device__ __forceinline__ void finish_rows(const GemvDesc& d, const float (&acc)[RMAX][MB], float bias, int n, int M, float res,
-                                            bool res_valid, int D, int Tmax, int pos, int lane) {
+// lanes [8r, 8r + MB) finish row n + r  (R <= RMAX = 4, MB <= 8); W8: the row's scale multiplies the dot product first
+template <int MB, unsigned VAR, bool W8>
+__device__ __forceinline__ void finish_rows(const GemvDesc& d, const float (&acc)[RMAX][MB], float scale, float bias, int n, int M,
+                                            float res, bool res_valid, int D, int Tmax, int pos, int lane) {
   const int m = lane & 7, r_sel = lane >> 3;
   const int nn = n + r_sel;
   if (r_sel < d.R && m < MB && m < M && nn < d.nend) {
@@ -319,6 +328,7 @@ __device__ __forceinline__ void finish_rows(const GemvDesc& d, const float (&acc
       for (int mm = 0; mm < MB; ++mm)
         if (r == r_sel && mm == m) v = acc[r][mm];
     }
+    if (W8) v *= scale;
     v += bias;
     if (nn < d.alpha_cols) v *= d.alpha;
     if (d.act == 1) v = gelu_erf(v);
@@ -333,9 +343,11 @@ __device__ __forceinline__ void finish_rows(const GemvDesc& d, const float (&acc
 }
 
 // smem carve-up (dynamic): red [64] | xs [MB*ffn] | pool: weight slabs from 0, attention scratch from ATT_OFF
-template <int MB, unsigned VAR>
+// W8: int8 decoder weights (1-byte slab rows, a scale per output row); the static smem is the same in both instantiations
+template <int MB, unsigned VAR, bool W8>
 __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constant__ MegaArgs a) {
   constexpr bool TRACE = !(VAR & V_NOTRACE);
+  constexpr int ESZ = W8 ? 1 : 2;
   extern __shared__ __align__(128) uint8_t dyn[];
   float* red = reinterpret_cast<float*>(dyn);
   float* xs = red + 64;
@@ -383,7 +395,7 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
 
   const int pos = pos0;
   // ---- phase 0: embedding (CTA 0 writes the residual stream); first QKV rows + LN1 params requested meanwhile
-  GemvDesc cur = make_desc<VAR>(a, sl, 0, 0, pos);
+  GemvDesc cur = make_desc<VAR, W8>(a, sl, 0, 0, pos);
   Pre pre;
   // Slab regions: GEMV phase ph (= 6*layer + g) lives in region ph & 1 -- region 1 at the pool's start (out-proj, cross
   // out-proj, fc2), region 0 at p0_off (QKV, cross-q, fc1).  Double-buffered (p0_off > 0), the copy for phase ph + 1 is
@@ -391,13 +403,16 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
   // requested just before the barrier left 0.3-1.3 us of L2 -> smem transfer exposed behind it).  Attention scratch starts
   // at ATT_OFF, above the small region-1 slabs that are live during the attention phases, and overlays region 0.
   const bool dbuf = a.p0_off > 0;
-  issue_slabs(cur, pool + a.p0_off, &cbar[0]);
-  prefetch_phase(cur, pre, pool, &wbar[warp], gw, warp, lane);
+  issue_slabs<ESZ>(cur, pool + a.p0_off, &cbar[0]);
+  prefetch_phase<W8>(cur, pre, pool, &wbar[warp], gw, warp, lane);
   if (blockIdx.x == 0) {
     for (int i = threadIdx.x; i < Q * D; i += MT) {
       const int q = i / D, d = i - q * D;
       const int tok = a.tokens[q * a.Tmax + pos];
-      a.dx[i] = e2f(a.embed[(long long)tok * D + d]) + a.dec_pos[(long long)pos * D + d];
+      if constexpr (W8)
+        a.dx[i] = a.embed_scale[tok] * (float)static_cast<const int8_t*>(a.embed)[(long long)tok * D + d] + a.dec_pos[(long long)pos * D + d];
+      else
+        a.dx[i] = e2f(static_cast<const bf16*>(a.embed)[(long long)tok * D + d]) + a.dec_pos[(long long)pos * D + d];
     }
   }
   bar.sync();
@@ -420,8 +435,8 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
       // phase the L2 prefetch of this layer's cross-attention K/V (DRAM -> L2, three phases before its bulk load)
       auto ahead = [&]() {
         if (dbuf && ph + 1 < nph) {
-          const GemvDesc d1 = make_desc<VAR>(a, sl, (ph + 1) / 6, (ph + 1) % 6, pos);
-          issue_slabs(d1, pool + (((ph + 1) & 1) ? 0 : a.p0_off), &cbar[(ph + 1) & 1]);
+          const GemvDesc d1 = make_desc<VAR, W8>(a, sl, (ph + 1) / 6, (ph + 1) % 6, pos);
+          issue_slabs<ESZ>(d1, pool + (((ph + 1) & 1) ? 0 : a.p0_off), &cbar[(ph + 1) & 1]);
         }
         if (g == 0 && threadIdx.x == DMA_T + 1 && blockIdx.x < Q * H * nsplit) {  // this layer's cross-attention item
           const int item = blockIdx.x;
@@ -440,13 +455,13 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
       if (active) {
         mbar_wait(&cbar[ph & 1], (ph & 1) ? cpar1 : cpar0);
         if (mkbase && lane == 0) wts[warp][0] = global_ns();
-        const uint8_t* slab = pool + ((ph & 1) ? 0 : a.p0_off) + (size_t)warp * cur.R * cur.K * 2;
+        const uint8_t* slab = pool + ((ph & 1) ? 0 : a.p0_off) + (size_t)warp * cur.R * cur.K * ESZ;
         float acc[RMAX][MB];
-        if (cur.R == 4) dot_rows<MB, 4>(slab, xs, cur.K, acc, lane);
-        else if (cur.R == 3) dot_rows<MB, 3>(slab, xs, cur.K, acc, lane);
-        else if (cur.R == 2) dot_rows<MB, 2>(slab, xs, cur.K, acc, lane);
-        else dot_rows<MB, 1>(slab, xs, cur.K, acc, lane);
-        finish_rows<MB, VAR>(cur, acc, pre.bias, n, Q, res, true, D, a.Tmax, pos, lane);
+        if (cur.R == 4) dot_rows<MB, 4, W8>(slab, xs, cur.K, acc, lane);
+        else if (cur.R == 3) dot_rows<MB, 3, W8>(slab, xs, cur.K, acc, lane);
+        else if (cur.R == 2) dot_rows<MB, 2, W8>(slab, xs, cur.K, acc, lane);
+        else dot_rows<MB, 1, W8>(slab, xs, cur.K, acc, lane);
+        finish_rows<MB, VAR, W8>(cur, acc, pre.scale, pre.bias, n, Q, res, true, D, a.Tmax, pos, lane);
         if (mkbase && lane == 0) wts[warp][1] = global_ns();
       }
       mark(3);
@@ -466,9 +481,9 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
       mkbase[bar.epoch * 4 + 0] = t0;
       mkbase[bar.epoch * 4 + 1] = t1;
     }
-    cur = make_desc<VAR>(a, sl, ph + 1 < nph ? (ph + 1) / 6 : a.L, (ph + 1) % 6, pos);
-    if (!dbuf && !cur.lm) issue_slabs(cur, pool, &cbar[(ph + 1) & 1]);
-    prefetch_phase(cur, pre, pool, &wbar[warp], gw, warp, lane);
+    cur = make_desc<VAR, W8>(a, sl, ph + 1 < nph ? (ph + 1) / 6 : a.L, (ph + 1) % 6, pos);
+    if (!dbuf && !cur.lm) issue_slabs<ESZ>(cur, pool, &cbar[(ph + 1) & 1]);
+    prefetch_phase<W8>(cur, pre, pool, &wbar[warp], gw, warp, lane);
 
     if (g == 0) {
       // past K/V rows of this CTA's self-attention item do not depend on this step: request them now
@@ -621,7 +636,7 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
   unsigned long long best = 0ull;  // of the logits this lane finished: (order-preserving value bits << 32) | ~token
   {
     const int K = cur.K, N = cur.N;
-    const size_t slab_bytes = (size_t)2 * K * 2;
+    const size_t slab_bytes = (size_t)2 * K * ESZ;
     const size_t set_bytes = slab_bytes * MW;
     int buf = 0;
     const bool at_begin = (pos + 1 == a.begin_index) && a.begin_suppress_bits;
@@ -629,8 +644,10 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
       const int n2 = n + GW * 2;
       if (n2 < N) {
         __syncwarp();  // every lane is done reading the stage that is refilled now
-        issue_rows(pool + (buf ^ 1) * set_bytes + (size_t)warp * slab_bytes, &wbar[(buf ^ 1) * MW + warp], cur.W, K, 2, n2, N, lane);
+        issue_rows<ESZ>(pool + (buf ^ 1) * set_bytes + (size_t)warp * slab_bytes, &wbar[(buf ^ 1) * MW + warp], cur.W, K, 2, n2, N, lane);
       }
+      float sc = 1.f;  // W8: scale of the row this lane finishes (requested before the slab wait)
+      if constexpr (W8) sc = cur.scale[min(n + (lane >> 3), N - 1)];
       if (buf == 0) {
         mbar_wait(&wbar[warp], wpar);
         wpar ^= 1u;
@@ -639,8 +656,8 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
         wpar1 ^= 1u;
       }
       float acc[RMAX][MB];
-      dot_rows<MB, 2>(pool + buf * set_bytes + (size_t)warp * slab_bytes, xs, K, acc, lane);
-      finish_rows<MB, VAR>(cur, acc, 0.f, n, Q, 0.f, true, D, a.Tmax, pos, lane);
+      dot_rows<MB, 2, W8>(pool + buf * set_bytes + (size_t)warp * slab_bytes, xs, K, acc, lane);
+      finish_rows<MB, VAR, W8>(cur, acc, sc, 0.f, n, Q, 0.f, true, D, a.Tmax, pos, lane);
       if (a.fuse_select) {
         const int m = lane & 7, r_sel = lane >> 3, nn = n + r_sel;
         if (r_sel < 2 && m < MB && m < Q && nn < N) {
@@ -650,6 +667,7 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
 #pragma unroll
             for (int mm = 0; mm < MB; ++mm)
               if (r == r_sel && mm == m) v = acc[r][mm];
+          if (W8) v *= sc;
           bool masked = (a.suppress_bits[nn >> 5] >> (nn & 31)) & 1u;
           if (at_begin) masked = masked || ((a.begin_suppress_bits[nn >> 5] >> (nn & 31)) & 1u);
           if (!masked) {
@@ -711,7 +729,7 @@ int g_mega_coop = -1;  // -1: read BW_MEGA_COOP on first use; the engine clears 
 
 namespace {
 
-template <int MB, unsigned VAR>
+template <int MB, unsigned VAR, bool W8>
 int launch_mega(cudaStream_t st, const MegaArgs& a, int num_sms, int coop) {
   // the shared-memory budget: the device's opt-in limit per block less this instantiation's static smem, read once
   static size_t limit = 0, attr = 0;
@@ -720,16 +738,16 @@ int launch_mega(cudaStream_t st, const MegaArgs& a, int num_sms, int coop) {
     BW_CUDA_OK(cudaGetDevice(&dev));
     BW_CUDA_OK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
     cudaFuncAttributes fa{};
-    BW_CUDA_OK(cudaFuncGetAttributes(&fa, decode_mega_kernel<MB, VAR>));
+    BW_CUDA_OK(cudaFuncGetAttributes(&fa, decode_mega_kernel<MB, VAR, W8>));
     limit = (size_t)optin - fa.sharedSizeBytes;
   }
   MegaArgs b = a;
-  const size_t smem = mega_smem_plan(MB, a.D, a.ffn, num_sms, !(a.flags & 2), limit, &b.p0_off);
+  const size_t smem = mega_smem_plan(MB, a.D, a.ffn, num_sms, !(a.flags & 2), limit, &b.p0_off, W8 ? 1 : 2);
   if (!smem) return -3;
   if (smem > attr) {
-    BW_CUDA_OK(cudaFuncSetAttribute(decode_mega_kernel<MB, VAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    BW_CUDA_OK(cudaFuncSetAttribute(decode_mega_kernel<MB, VAR, W8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;
-    BW_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_mega_kernel<MB, VAR>, MT, smem));
+    BW_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_mega_kernel<MB, VAR, W8>, MT, smem));
     if (per_sm < 1) return -3;
     attr = smem;
   }
@@ -739,7 +757,7 @@ int launch_mega(cudaStream_t st, const MegaArgs& a, int num_sms, int coop) {
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
   cfg.attrs = at; cfg.numAttrs = coop ? 1 : 0;
-  BW_CUDA_OK(cudaLaunchKernelEx(&cfg, decode_mega_kernel<MB, VAR>, b));
+  BW_CUDA_OK(cudaLaunchKernelEx(&cfg, decode_mega_kernel<MB, VAR, W8>, b));
   return 0;
 }
 
@@ -749,14 +767,16 @@ int launch_mega(cudaStream_t st, const MegaArgs& a, int num_sms, int coop) {
 // (the caller then uses the per-op path).
 int launch_decode_mega(cudaStream_t st, const MegaArgs& a, int num_sms) {
   const int Q = a.Q;
+  const bool w8 = a.embed_scale != nullptr;
+  const size_t esz = w8 ? 1 : 2;
   if (a.L > MEGA_MAXL || Q > 2 || a.D > MAXD || a.ffn > 5120 || a.D % 8 != 0 || a.ffn % 8 != 0 || a.Tmax > MAXKEYS) return -3;
-  if ((size_t)MW * a.D * 2 > (size_t)ATT_OFF) return -3;  // R=1 slabs must stay below the attention scratch
+  if ((size_t)MW * a.D * esz > (size_t)ATT_OFF) return -3;  // R=1 slabs must stay below the attention scratch
   {  // every layer GEMV is one pass of at most RMAX rows per warp
     const int nmax = 3 * a.D > a.ffn ? 3 * a.D : a.ffn;
     if (((nmax + num_sms - 1) / num_sms + MW - 1) / MW > RMAX) return -3;
   }
   if (a.nsplit > XSPLIT) return -3;
-  if ((size_t)((a.D + num_sms - 1) / num_sms) * a.D * 2 > (size_t)ATT_OFF) return -3;  // region-1 slabs live under the attention scratch
+  if ((size_t)((a.D + num_sms - 1) / num_sms) * a.D * esz > (size_t)ATT_OFF) return -3;  // region-1 slabs live under the attention scratch
   const int ks = (a.S + a.nsplit - 1) / a.nsplit;
   if (ks > XKMAX) return -3;
   // Co-residency of the CTAs (one per SM) (round-1 advisor): the grid barriers spin, so a CTA that is not scheduled deadlocks the rest until
@@ -770,8 +790,13 @@ int launch_decode_mega(cudaStream_t st, const MegaArgs& a, int num_sms) {
   }
   // the instrumented instantiation only when a trace buffer is attached (BW_MEGA_TRACE=1)
   int rc;
-  if (Q <= 1) rc = a.trace ? launch_mega<1, 0u>(st, a, num_sms, coop) : launch_mega<1, V_NOTRACE>(st, a, num_sms, coop);
-  else rc = a.trace ? launch_mega<2, 0u>(st, a, num_sms, coop) : launch_mega<2, V_NOTRACE>(st, a, num_sms, coop);
+  if (w8) {
+    if (Q <= 1) rc = a.trace ? launch_mega<1, 0u, true>(st, a, num_sms, coop) : launch_mega<1, V_NOTRACE, true>(st, a, num_sms, coop);
+    else rc = a.trace ? launch_mega<2, 0u, true>(st, a, num_sms, coop) : launch_mega<2, V_NOTRACE, true>(st, a, num_sms, coop);
+  } else {
+    if (Q <= 1) rc = a.trace ? launch_mega<1, 0u, false>(st, a, num_sms, coop) : launch_mega<1, V_NOTRACE, false>(st, a, num_sms, coop);
+    else rc = a.trace ? launch_mega<2, 0u, false>(st, a, num_sms, coop) : launch_mega<2, V_NOTRACE, false>(st, a, num_sms, coop);
+  }
   if (rc) return rc;
   BW_CUDA_OK(cudaGetLastError());
   return 0;

@@ -57,13 +57,16 @@ __device__ __forceinline__ long long global_ns() {
   return t;
 }
 
-__device__ __forceinline__ void issue_rows(uint8_t* slab, uint64_t* bar, const bf16* W, int K, int R, int n, int N, int lane) {
+// W: rows of K elements of ESZ bytes (2: the engine's 16-bit type, 1: int8 codes)
+template <int ESZ>
+__device__ __forceinline__ void issue_rows(uint8_t* slab, uint64_t* bar, const uint8_t* W, int K, int R, int n, int N, int lane) {
   if (lane == 0) {
-    const uint32_t row_bytes = (uint32_t)K * 2;
+    const uint32_t row_bytes = (uint32_t)K * ESZ;
     mbar_arrive_expect_tx(bar, row_bytes * R);
     for (int r = 0; r < R; ++r) {
       const int row = min(n + r, N - 1);
-      bulk_g2s(slab + (size_t)r * row_bytes, W + (long long)row * K, row_bytes, bar);
+      if constexpr (ESZ == 2) bulk_g2s(slab + (size_t)r * row_bytes, reinterpret_cast<const bf16*>(W) + (long long)row * K, row_bytes, bar);
+      else bulk_g2s(slab + (size_t)r * row_bytes, W + (long long)row * K, row_bytes, bar);
     }
   }
 }
@@ -72,7 +75,8 @@ __device__ __forceinline__ void issue_rows(uint8_t* slab, uint64_t* bar, const b
 __device__ __forceinline__ void l2_prefetch(const void* p, uint32_t bytes) {
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
 }
-template <int MB, int R>
+// W8: int8 rows -- a lane reads 4 codes (4 B) at the same k0, so 32 lanes read 128 contiguous bytes (conflict-free)
+template <int MB, int R, bool W8>
 __device__ __forceinline__ void dot_chunk(const uint8_t* slab, const float* xs, int K, int k0, bool hi, float (&s)[R][MB]) {
   float4 x0[MB], x1[MB];
 #pragma unroll
@@ -82,9 +86,19 @@ __device__ __forceinline__ void dot_chunk(const uint8_t* slab, const float* xs, 
   }
 #pragma unroll
   for (int r = 0; r < R; ++r) {
-    const uint2 wa = *reinterpret_cast<const uint2*>(slab + ((size_t)r * K + k0) * 2);
-    const uint2 wc = hi ? *reinterpret_cast<const uint2*>(slab + ((size_t)r * K + k0 + 128) * 2) : make_uint2(0u, 0u);
-    const float2 a0 = unpack_bf16(wa.x), a1 = unpack_bf16(wa.y), c0 = unpack_bf16(wc.x), c1 = unpack_bf16(wc.y);
+    float2 a0, a1, c0, c1;
+    if constexpr (W8) {
+      const uint32_t wa = *reinterpret_cast<const uint32_t*>(slab + (size_t)r * K + k0);
+      const uint32_t wc = hi ? *reinterpret_cast<const uint32_t*>(slab + (size_t)r * K + k0 + 128) : 0u;
+      float fa[4], fc[4];
+      unpack_s8x4(wa, fa);
+      unpack_s8x4(wc, fc);
+      a0 = make_float2(fa[0], fa[1]); a1 = make_float2(fa[2], fa[3]); c0 = make_float2(fc[0], fc[1]); c1 = make_float2(fc[2], fc[3]);
+    } else {
+      const uint2 wa = *reinterpret_cast<const uint2*>(slab + ((size_t)r * K + k0) * 2);
+      const uint2 wc = hi ? *reinterpret_cast<const uint2*>(slab + ((size_t)r * K + k0 + 128) * 2) : make_uint2(0u, 0u);
+      a0 = unpack_bf16(wa.x); a1 = unpack_bf16(wa.y); c0 = unpack_bf16(wc.x); c1 = unpack_bf16(wc.y);
+    }
 #pragma unroll
     for (int m = 0; m < MB; ++m) {
       float t = s[r][m], u = 0.f;
@@ -100,7 +114,7 @@ __device__ __forceinline__ void dot_chunk(const uint8_t* slab, const float* xs, 
 // The full 256-element chunks run branch-free (unrolled by 5 so the loads of several chunks are in flight together: with a
 // guard per chunk the compiler serialised load -> convert -> FMA chunk by chunk, ~120 cycles each); a ragged tail
 // (K % 256 != 0: only the small test models) takes the guarded path.
-template <int MB, int R>
+template <int MB, int R, bool W8>
 __device__ __forceinline__ void dot_rows(const uint8_t* slab, const float* xs, int K, float (&acc)[RMAX][MB], int lane) {
   float s[R][MB];
 #pragma unroll
@@ -110,8 +124,8 @@ __device__ __forceinline__ void dot_rows(const uint8_t* slab, const float* xs, i
   const int nfull = K >> 8;
   int k0 = lane * 4;
 #pragma unroll 5
-  for (int c = 0; c < nfull; ++c, k0 += 256) dot_chunk<MB, R>(slab, xs, K, k0, true, s);
-  if (k0 < K) dot_chunk<MB, R>(slab, xs, K, k0, (k0 + 128) < K, s);
+  for (int c = 0; c < nfull; ++c, k0 += 256) dot_chunk<MB, R, W8>(slab, xs, K, k0, true, s);
+  if (k0 < K) dot_chunk<MB, R, W8>(slab, xs, K, k0, (k0 + 128) < K, s);
 #pragma unroll
   for (int r = 0; r < RMAX; ++r)
 #pragma unroll
@@ -254,8 +268,11 @@ __device__ __forceinline__ void attend_smem(const uint8_t* sK, const uint8_t* sV
 // smem plan: returns the dynamic smem bytes (0: does not fit in `limit`) and the offset of slab region 0 (0: single-buffered,
 // everything at the pool's start).  limit = the device's opt-in shared memory per block less the kernel's static smem (layer
 // table, barriers): on 132 SMs the double-buffered plan for large-v3 at Q = 1 fits with a few hundred bytes to spare, so the
-// limit is taken from the device and the compiled kernel, not estimated.
-inline size_t mega_smem_plan(int mb, int D, int ffn, int num_sms, bool want_dbuf, size_t limit, int* p0_off) {
+// limit is taken from the device and the compiled kernel, not estimated.  esz: bytes per weight element (2, or 1 for int8).
+// The overlap rule does not depend on esz: during an attention phase only the out-proj / cross out-proj slabs (K = D) of
+// region 1 are live, and they stay below ATT_OFF (the launcher checks it for the element size); the attention scratch itself
+// does not shrink with the weights, so with 1-byte rows it, not the slab regions, bounds the pool.
+inline size_t mega_smem_plan(int mb, int D, int ffn, int num_sms, bool want_dbuf, size_t limit, int* p0_off, int esz = 2) {
   // rows of a CTA, rounded up to whole active warps: the unused rows of the last active warp are still read (and discarded)
   auto rc = [&](int n) {
     const int rows = (n + num_sms - 1) / num_sms, R = (rows + MW - 1) / MW;
@@ -264,12 +281,12 @@ inline size_t mega_smem_plan(int mb, int D, int ffn, int num_sms, bool want_dbuf
   const size_t attn = (size_t)MAXKEYS * 256 + (size_t)(MW * 72) * sizeof(float);
   const size_t xattn = (size_t)2 * XKMAX * 128 + (size_t)(MW * 72) * sizeof(float);
   const size_t att = ATT_OFF + (attn > xattn ? attn : xattn);
-  const size_t lm = (size_t)MW * 2 * 2 * D * 2;  // LM head: 2 stages of row pairs per warp
-  size_t r1 = rc(D) * ffn * 2;                   // region 1: out-proj / cross out-proj (K = D), fc2 (K = ffn)
-  if (rc(D) * D * 2 > r1) r1 = rc(D) * D * 2;
-  size_t r0 = rc(3 * D) * D * 2;                 // region 0: QKV, cross-q, fc1
-  if (rc(ffn) * D * 2 > r0) r0 = rc(ffn) * D * 2;
-  if (rc(D) * D * 2 > r0) r0 = rc(D) * D * 2;
+  const size_t lm = (size_t)MW * 2 * 2 * D * esz;  // LM head: 2 stages of row pairs per warp
+  size_t r1 = rc(D) * ffn * esz;                   // region 1: out-proj / cross out-proj (K = D), fc2 (K = ffn)
+  if (rc(D) * D * esz > r1) r1 = rc(D) * D * esz;
+  size_t r0 = rc(3 * D) * D * esz;                 // region 0: QKV, cross-q, fc1
+  if (rc(ffn) * D * esz > r0) r0 = rc(ffn) * D * esz;
+  if (rc(D) * D * esz > r0) r0 = rc(D) * D * esz;
   const size_t fixed = 64 * sizeof(float) + (size_t)mb * ffn * sizeof(float) + 128;
   auto mx = [](size_t a, size_t b) { return a > b ? a : b; };
   const size_t off = (r1 + 127) / 128 * 128;

@@ -7,6 +7,8 @@
 // then computes.  (A first version looped load->use with 4-8 loads in flight and reached a small fraction of the HBM roofline.)
 #include <math.h>
 
+#include <type_traits>
+
 #include "decode.cuh"
 #include "kernels.h"
 
@@ -70,22 +72,37 @@ __device__ __forceinline__ void split_sum8(const float* __restrict__ p, long lon
   o[0] = a0.x; o[1] = a0.y; o[2] = a0.z; o[3] = a0.w; o[4] = a1.x; o[5] = a1.y; o[6] = a1.z; o[7] = a1.w;
 }
 
-template <int NC, int R>
+// W8: int8 weight codes, 8 per lane and chunk in one 8-byte load (the same k -> lane map as the 16-bit rows, so the x reads
+// from smem stay conflict-free; a warp-load is 256 contiguous bytes)
+template <int NC, int R, bool W8>
 struct WRegs {
-  uint4 w[R][NC];
+  typename std::conditional<W8, uint2, uint4>::type w[R][NC];
 };
 
+__device__ __forceinline__ void unpack8(const uint2& u, float (&f)[8]) {
+  float a[4], b[4];
+  unpack_s8x4(u.x, a);
+  unpack_s8x4(u.y, b);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) { f[i] = a[i]; f[4 + i] = b[i]; }
+}
+
 // lane l holds elements [l*8 + i*256, +8) of each row, i < NC  (512 contiguous bytes per warp-load: fully coalesced)
-template <int NC, int R>
-__device__ __forceinline__ void load_rows(WRegs<NC, R>& wr, const bf16* __restrict__ W, int K, int n, int n_end, int lane) {
+template <int NC, int R, bool W8>
+__device__ __forceinline__ void load_rows(WRegs<NC, R, W8>& wr, const void* __restrict__ W, int K, int n, int n_end, int lane) {
 #pragma unroll
   for (int r = 0; r < R; ++r) {
     const int row = min(n + r, n_end - 1);  // clamp: a duplicate row whose result is discarded
-    const bf16* wp = W + (long long)row * K;
 #pragma unroll
     for (int i = 0; i < NC; ++i) {
       const int k = lane * 8 + i * 256;
-      wr.w[r][i] = (k < K) ? ld_nc_u4(wp + k) : make_uint4(0u, 0u, 0u, 0u);
+      if constexpr (W8) {
+        const int8_t* wp = static_cast<const int8_t*>(W) + (long long)row * K;
+        wr.w[r][i] = (k < K) ? ld_nc_u2(wp + k) : make_uint2(0u, 0u);
+      } else {
+        const bf16* wp = static_cast<const bf16*>(W) + (long long)row * K;
+        wr.w[r][i] = (k < K) ? ld_nc_u4(wp + k) : make_uint4(0u, 0u, 0u, 0u);
+      }
     }
   }
 }
@@ -93,7 +110,7 @@ __device__ __forceinline__ void load_rows(WRegs<NC, R>& wr, const bf16* __restri
 // ------------------------------------------------------------------------------------------------
 // out[m, n] = epi( LN?(x[m, :]) . W[n, :] ), m < MB <= 8.  NC = ceil(K / 256) bound, R rows per warp in flight.
 // ------------------------------------------------------------------------------------------------
-template <int MB, int NC, int R, bool PIPE>
+template <int MB, int NC, int R, bool PIPE, bool W8>
 __global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(const GemvArgs a, const int rows_per_warp) {
   extern __shared__ float xs[];  // [MB][K]
   __shared__ float red[GEMV_WARPS][MB];
@@ -105,8 +122,8 @@ __global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(const GemvArgs a, co
   const int n_end = min(a.N, n_begin + rows_per_warp);
 
   // 1) weight rows of the first pass: requested before anything else so the DRAM latency hides the prologue
-  WRegs<NC, R> cur;
-  if (n_begin < n_end) load_rows<NC, R>(cur, a.W, K, n_begin, n_end, lane);
+  WRegs<NC, R, W8> cur;
+  if (n_begin < n_end) load_rows<NC, R, W8>(cur, a.W, K, n_begin, n_end, lane);
 
   // 2) for every chunk of MB rows of x: stage (+ LayerNorm: two-pass, biased variance, eps 1e-5 like torch.nn.LayerNorm),
   //    then all of this warp's weight rows against the chunk.  M > MB re-uses the weights already in registers, so a
@@ -169,12 +186,13 @@ __global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(const GemvArgs a, co
       }
       __syncthreads();
     }
-    // (multi-pass launches -- the LM head -- are only issued with M <= MB, so `cur` is reloaded per chunk only then)
-    if (m0 > 0 && !single_pass && n_begin < n_end) load_rows<NC, R>(cur, a.W, K, n_begin, n_end, lane);
+    // a warp with more rows than one pass (the LM head) reloads its first rows for every chunk of MB sequences: with M > MB its
+    // weights are streamed ceil(M / MB) times per launch (the batched step, not this kernel, serves large M by default)
+    if (m0 > 0 && !single_pass && n_begin < n_end) load_rows<NC, R, W8>(cur, a.W, K, n_begin, n_end, lane);
     for (int n = n_begin; n < n_end; n += R) {
-      WRegs<NC, R> nxt;
+      WRegs<NC, R, W8> nxt;
       const bool has_next = (n + R) < n_end;
-      if (PIPE && has_next) load_rows<NC, R>(nxt, a.W, K, n + R, n_end, lane);
+      if (PIPE && has_next) load_rows<NC, R, W8>(nxt, a.W, K, n + R, n_end, lane);
       float acc[R][MB];
 #pragma unroll
       for (int r = 0; r < R; ++r)
@@ -216,6 +234,7 @@ __global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(const GemvArgs a, co
           for (int mm = 0; mm < MB; ++mm)
             if (r == r_sel && mm == m) v = acc[r][mm];
         const int mg = m0 + m;
+        if (W8) v *= a.wscale[nn];
         if (a.bias) v += a.bias[nn];
         if (nn < a.alpha_cols) v *= a.alpha;
         if (a.act == 1) v = gelu_erf(v);
@@ -230,7 +249,7 @@ __global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(const GemvArgs a, co
       if (PIPE) {
         if (has_next) cur = nxt;
       } else if (has_next) {
-        load_rows<NC, R>(cur, a.W, K, n + R, n_end, lane);
+        load_rows<NC, R, W8>(cur, a.W, K, n + R, n_end, lane);
       }
     }
   }
@@ -707,19 +726,19 @@ __global__ void __launch_bounds__(128) cross_attn_stream_kernel(const CrossAttnA
   }
 }
 
-template <int MB, int NC, int R, bool PIPE>
+template <int MB, int NC, int R, bool PIPE, bool W8>
 int launch_gemv_t(cudaStream_t st, const GemvArgs& a, int grid, int rpw, size_t smem) {
   static bool attr = false;
   if (!attr) {
-    BW_CUDA_OK(cudaFuncSetAttribute(gemv_kernel<MB, NC, R, PIPE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    BW_CUDA_OK(cudaFuncSetAttribute(gemv_kernel<MB, NC, R, PIPE, W8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     attr = true;
   }
-  gemv_kernel<MB, NC, R, PIPE><<<grid, GEMV_THREADS, smem, st>>>(a, rpw);
+  gemv_kernel<MB, NC, R, PIPE, W8><<<grid, GEMV_THREADS, smem, st>>>(a, rpw);
   BW_CUDA_OK(cudaGetLastError());
   return 0;
 }
 
-template <int MB>
+template <int MB, bool W8>
 int launch_gemv_mb(cudaStream_t st, const GemvArgs& a) {
   const size_t smem = (size_t)MB * a.K * sizeof(float);
   if (a.K <= 1280) {
@@ -728,13 +747,21 @@ int launch_gemv_mb(cudaStream_t st, const GemvArgs& a) {
     rpw = (rpw + 1) & ~1;
     if (rpw < 2) rpw = 2;
     const int grid = (a.N + rpw * GEMV_WARPS - 1) / (rpw * GEMV_WARPS);
-    return launch_gemv_t<MB, 5, 2, true>(st, a, grid, rpw, smem);
+    return launch_gemv_t<MB, 5, 2, true, W8>(st, a, grid, rpw, smem);
   }
   // long rows (fc2, K = 4*D): one row per warp, all 20 loads of the row in flight
   int rpw = (a.N + 592 * GEMV_WARPS - 1) / (592 * GEMV_WARPS);
   if (rpw < 1) rpw = 1;
   const int grid = (a.N + rpw * GEMV_WARPS - 1) / (rpw * GEMV_WARPS);
-  return launch_gemv_t<MB, 20, 1, false>(st, a, grid, rpw, smem);
+  return launch_gemv_t<MB, 20, 1, false, W8>(st, a, grid, rpw, smem);
+}
+
+template <bool W8>
+int launch_gemv_w(cudaStream_t st, const GemvArgs& a) {
+  if (a.M <= 1) return launch_gemv_mb<1, W8>(st, a);
+  if (a.M <= 2) return launch_gemv_mb<2, W8>(st, a);
+  if (a.M <= 4) return launch_gemv_mb<4, W8>(st, a);
+  return launch_gemv_mb<8, W8>(st, a);  // M > 8: the kernel walks the rows in chunks of 8 with the weights held in registers
 }
 
 }  // namespace
@@ -742,10 +769,7 @@ int launch_gemv_mb(cudaStream_t st, const GemvArgs& a) {
 int launch_gemv(cudaStream_t st, const GemvArgs& a) {
   BW_CHECK(a.M >= 1, "gemv: M=%d must be >= 1", a.M);
   BW_CHECK(a.K % 8 == 0 && a.K <= 5120, "gemv: K=%d must be a multiple of 8 and <= 5120", a.K);
-  if (a.M <= 1) return launch_gemv_mb<1>(st, a);
-  if (a.M <= 2) return launch_gemv_mb<2>(st, a);
-  if (a.M <= 4) return launch_gemv_mb<4>(st, a);
-  return launch_gemv_mb<8>(st, a);  // M > 8: the kernel walks the rows in chunks of 8 with the weights held in registers
+  return a.wscale ? launch_gemv_w<true>(st, a) : launch_gemv_w<false>(st, a);
 }
 
 int launch_self_attn(cudaStream_t st, const SelfAttnArgs& a, int Q) {

@@ -278,6 +278,21 @@ int make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_
   return 0;
 }
 
+int make_tmap_2d_u8(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t row_pitch_bytes, uint32_t box_rows,
+                    uint32_t box_cols) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (!fn) return -1;
+  cuuint64_t dims[2] = {cols, rows};
+  cuuint64_t strides[1] = {row_pitch_bytes};
+  cuuint32_t box[2] = {box_cols, box_rows};
+  cuuint32_t es[2] = {1, 1};
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  BW_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(2d u8 rows=%llu cols=%llu pitch=%llu box=%ux%u) -> %d",
+           (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)row_pitch_bytes, box_rows, box_cols, (int)r);
+  return 0;
+}
+
 static int make_tmap_3d_bf16(CUtensorMap* out, const void* base, uint64_t batch, uint64_t rows, uint64_t cols,
                              uint64_t row_pitch_bytes, uint64_t batch_pitch_bytes, uint32_t box_rows, uint32_t box_cols) {
   EncodeTiledFn fn = get_encode_fn();

@@ -63,9 +63,10 @@ struct DecGemmPlan {
   int QB = 16, q_tiles = 1, stages = 2, kper = 1, ksplit = 1;
   size_t smem = 0;
 };
-DecGemmPlan gemm_dec_plan(int Q, int N, int K, int num_sms, bool want_split);
-int gemm_dec(cudaStream_t st, const bf16* X, const bf16* W, int Q, int N, int K, int n_valid, const GemmEpi& epi, const DecGemmPlan& pl,
-             long long split_stride);
+DecGemmPlan gemm_dec_plan(int Q, int N, int K, int num_sms, bool want_split, bool w8 = false);
+// W: [N, K] 16-bit, or int8 codes with a scale per row (wscale != nullptr; plan with w8 = true)
+int gemm_dec(cudaStream_t st, const bf16* X, const void* W, const float* wscale, int Q, int N, int K, int n_valid, const GemmEpi& epi,
+             const DecGemmPlan& pl, long long split_stride);
 // h[q, n] = bf16(GELU(sum_s part[s][q][n] + bias[n]))
 int launch_gelu_bias(cudaStream_t st, const float* part, int nsplit, long long split_stride, const float* bias, bf16* h, int Q, int N);
 

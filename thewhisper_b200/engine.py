@@ -63,6 +63,26 @@ def interpolate_positions(table: torch.Tensor, chunk_length_s: float) -> torch.T
 
 ENGINE_DTYPES = {torch.bfloat16: 0, torch.float16: 1}
 
+# The decoder matrices every step streams: per layer (engine names) and the tied embedding / LM head.  With
+# decoder_weights="int8" these are int8 codes with an fp32 scale per output row ("<name>.scale"); xwk / xwv stay 16-bit.
+INT8_LAYER_KINDS = ("wqkv", "wo", "xwq", "xwo", "w1", "w2")
+DECODER_WEIGHTS = (None, "int8")
+
+
+def quantize_rows(W: torch.Tensor):
+    """Per-row symmetric int8: s = amax(|w|, dim=1) / 127 (an all-zero row gets s = 1), q = clamp(round_half_even(w / s),
+    -127, 127).  -> (q int8 [N, K], s fp32 [N]); the weight the kernels compute with is exactly s[n] * q[n, k]."""
+    w = W.detach().float()
+    s = w.abs().amax(dim=1) / 127.0
+    s = torch.where(s == 0, torch.ones_like(s), s)
+    q = torch.clamp(torch.round(w / s[:, None]), -127, 127).to(torch.int8)  # torch.round rounds half to even
+    return q.contiguous(), s.contiguous()
+
+
+def decoder_weights_of(weights: Dict[str, torch.Tensor]) -> Optional[str]:
+    """The decoder-weight format of a packed weight dict: "int8" when it holds "dec.embed.scale", else None."""
+    return "int8" if "dec.embed.scale" in weights else None
+
 
 def engine_dtype(torch_dtype) -> torch.dtype:
     """The 16-bit element type the engine runs for a caller's `torch_dtype` (REF nvidia/asr_pipeline.py:39: None = the checkpoint's
@@ -72,14 +92,24 @@ def engine_dtype(torch_dtype) -> torch.dtype:
 
 
 def pack_weights(sd: Dict[str, torch.Tensor], dims: ModelDims, enc_pos: torch.Tensor, device: torch.device,
-                 dtype: torch.dtype = torch.bfloat16) -> Dict[str, torch.Tensor]:
+                 dtype: torch.dtype = torch.bfloat16, decoder_weights: Optional[str] = None) -> Dict[str, torch.Tensor]:
     """HF WhisperForConditionalGeneration state_dict -> named device tensors in the engine's layouts
-    (16-bit [out, in] matrices in `dtype`, fp32 vectors; q/k/v fused; conv kernels reordered to [co][tap][ci])."""
+    (16-bit [out, in] matrices in `dtype`, fp32 vectors; q/k/v fused; conv kernels reordered to [co][tap][ci]).
+    decoder_weights="int8": dec.embed and the decoder layers' wqkv / wo / xwq / xwo / w1 / w2 are packed as int8 codes plus
+    "<name>.scale" (quantize_rows of the checkpoint's values, on the device), with no 16-bit copy."""
+    if decoder_weights not in DECODER_WEIGHTS:
+        raise ValueError(f"decoder_weights must be one of {DECODER_WEIGHTS}, got {decoder_weights!r}")
     D = dims.d_model
     out: Dict[str, torch.Tensor] = {}
 
     def mat(t):
         return t.detach().to(device=device, dtype=dtype).contiguous()
+
+    def dmat(name, t):  # a matrix every decoder step streams
+        if decoder_weights == "int8":
+            out[name], out[name + ".scale"] = quantize_rows(t.detach().to(device=device))
+        else:
+            out[name] = mat(t)
 
     def vec(t):
         return t.detach().to(device=device, dtype=torch.float32).contiguous()
@@ -110,7 +140,7 @@ def pack_weights(sd: Dict[str, torch.Tensor], dims: ModelDims, enc_pos: torch.Te
         out[o + "w2"] = mat(sd[p + "fc2.weight"])
         out[o + "b2"] = vec(sd[p + "fc2.bias"])
     d = "model.decoder."
-    out["dec.embed"] = mat(sd[d + "embed_tokens.weight"])
+    dmat("dec.embed", sd[d + "embed_tokens.weight"])
     out["dec.pos"] = vec(sd[d + "embed_positions.weight"])
     out["dec.lnf.g"] = vec(sd[d + "layer_norm.weight"])
     out["dec.lnf.b"] = vec(sd[d + "layer_norm.bias"])
@@ -118,37 +148,42 @@ def pack_weights(sd: Dict[str, torch.Tensor], dims: ModelDims, enc_pos: torch.Te
         p, o = f"{d}layers.{i}.", f"dec.{i}."
         out[o + "ln1.g"] = vec(sd[p + "self_attn_layer_norm.weight"])
         out[o + "ln1.b"] = vec(sd[p + "self_attn_layer_norm.bias"])
-        out[o + "wqkv"] = mat(torch.cat([sd[p + "self_attn.q_proj.weight"], sd[p + "self_attn.k_proj.weight"],
-                                         sd[p + "self_attn.v_proj.weight"]], 0))
+        dmat(o + "wqkv", torch.cat([sd[p + "self_attn.q_proj.weight"], sd[p + "self_attn.k_proj.weight"],
+                                    sd[p + "self_attn.v_proj.weight"]], 0))
         out[o + "bqkv"] = vec(torch.cat([sd[p + "self_attn.q_proj.bias"].float().cpu(), zeros,
                                          sd[p + "self_attn.v_proj.bias"].float().cpu()], 0))
-        out[o + "wo"] = mat(sd[p + "self_attn.out_proj.weight"])
+        dmat(o + "wo", sd[p + "self_attn.out_proj.weight"])
         out[o + "bo"] = vec(sd[p + "self_attn.out_proj.bias"])
         out[o + "ln2.g"] = vec(sd[p + "encoder_attn_layer_norm.weight"])
         out[o + "ln2.b"] = vec(sd[p + "encoder_attn_layer_norm.bias"])
-        out[o + "xwq"] = mat(sd[p + "encoder_attn.q_proj.weight"])
+        dmat(o + "xwq", sd[p + "encoder_attn.q_proj.weight"])
         out[o + "xbq"] = vec(sd[p + "encoder_attn.q_proj.bias"])
         out[o + "xwk"] = mat(sd[p + "encoder_attn.k_proj.weight"])
         out[o + "xwv"] = mat(sd[p + "encoder_attn.v_proj.weight"])
         out[o + "xbv"] = vec(sd[p + "encoder_attn.v_proj.bias"])
-        out[o + "xwo"] = mat(sd[p + "encoder_attn.out_proj.weight"])
+        dmat(o + "xwo", sd[p + "encoder_attn.out_proj.weight"])
         out[o + "xbo"] = vec(sd[p + "encoder_attn.out_proj.bias"])
         out[o + "ln3.g"] = vec(sd[p + "final_layer_norm.weight"])
         out[o + "ln3.b"] = vec(sd[p + "final_layer_norm.bias"])
-        out[o + "w1"] = mat(sd[p + "fc1.weight"])
+        dmat(o + "w1", sd[p + "fc1.weight"])
         out[o + "b1"] = vec(sd[p + "fc1.bias"])
-        out[o + "w2"] = mat(sd[p + "fc2.weight"])
+        dmat(o + "w2", sd[p + "fc2.weight"])
         out[o + "b2"] = vec(sd[p + "fc2.bias"])
     return out
 
 
 class WhisperEngine:
-    """Native engine for one GPU.  `state_dict` is an HF Whisper checkpoint (container of weights only)."""
+    """Native engine for one GPU.  `state_dict` is an HF Whisper checkpoint (container of weights only).
+    decoder_weights="int8" stores the decoder matrices every step streams as int8 with a scale per row (see pack_weights);
+    a preloaded `weights` dict carries its own format (decoder_weights_of)."""
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], dims: ModelDims, chunk_length_s: float = 30,
                  device: str = "cuda:0", max_audios: int = 1, max_beams: int = 1,
                  alignment_heads: Optional[Sequence[Sequence[int]]] = None, max_align_steps: int = 448,
-                 weights: Optional[Dict[str, torch.Tensor]] = None, dtype: torch.dtype = torch.bfloat16):
+                 weights: Optional[Dict[str, torch.Tensor]] = None, dtype: torch.dtype = torch.bfloat16,
+                 decoder_weights: Optional[str] = None):
+        if decoder_weights not in DECODER_WEIGHTS:
+            raise ValueError(f"decoder_weights must be one of {DECODER_WEIGHTS}, got {decoder_weights!r}")
         self.lib = _lib.load()
         if not torch.cuda.is_available() or self.lib.bw_device_count() == 0:
             raise _lib.BwError("no CUDA device visible: thewhisper_b200 has no CPU fallback")
@@ -166,8 +201,11 @@ class WhisperEngine:
         if weights is None:
             table = state_dict["model.encoder.embed_positions.weight"]
             enc_pos = table.detach().float().cpu() if table.shape[0] == S else interpolate_positions(table, chunk_length_s)
-            weights = pack_weights(state_dict, dims, enc_pos, self.device, dtype)
-        else:  # preloaded: the matrices decide (all 16-bit tensors share one type)
+            weights = pack_weights(state_dict, dims, enc_pos, self.device, dtype, decoder_weights)
+        else:  # preloaded: the matrices decide (all 16-bit tensors share one type), "dec.embed.scale" the decoder format
+            if decoder_weights is not None and decoder_weights_of(weights) != decoder_weights:
+                raise _lib.BwError(f"decoder_weights={decoder_weights!r} but the preloaded weights hold "
+                                   f"{decoder_weights_of(weights) or '16-bit'} decoder matrices")
             mats = {t.dtype for t in weights.values() if t.dtype in ENGINE_DTYPES}
             if len(mats) != 1:
                 raise _lib.BwError(f"preloaded weights must hold matrices of exactly one 16-bit type, got {mats}")
@@ -175,6 +213,7 @@ class WhisperEngine:
         if dtype not in ENGINE_DTYPES:
             raise _lib.BwError(f"engine dtype must be torch.bfloat16 or torch.float16, got {dtype}")
         self.dtype = dtype
+        self.decoder_weights = decoder_weights_of(weights)
         self.weights = weights  # keeps the device memory alive
         cfg = _lib.bw_config(dims.d_model, dims.n_heads, dims.ffn, dims.enc_layers, dims.dec_layers, dims.n_mels,
                              dims.vocab, S, dims.max_target_positions, max_audios, max_beams,

@@ -30,7 +30,11 @@ from ..hostproc import AsrDecoder, chunk_windows, install_merge
 
 class ASRPipeline:
     def __init__(self, model, feature_extractor=None, tokenizer=None, model_size: Optional[str] = None,
-                 chunk_length_s: int = 30, device: str = "cuda", torch_dtype: Optional[torch.dtype] = None, **kwargs):
+                 chunk_length_s: int = 30, device: str = "cuda", torch_dtype: Optional[torch.dtype] = None,
+                 decoder_weights: Optional[str] = None, **kwargs):
+        # decoder_weights="int8": the decoder matrices every step streams are held as int8 with an fp32 scale per row
+        # (WhisperEngine / pack_weights); None keeps them in the engine's 16-bit type.  Independent of `model_size`.
+        self.decoder_weights = decoder_weights
         revision = kwargs.pop("revision", "main")
         self.batch_size = int(kwargs.pop("batch_size", 1) or 1)
         self.max_beams = int(kwargs.pop("max_beams", 5))
@@ -95,7 +99,8 @@ class ASRPipeline:
             self.engine.close()
         self.engine = WhisperEngine(self._state_dict, self.dims, chunk_length_s=self.chunk_length_s, device=self.device,
                                     max_audios=capacity, max_beams=self.max_beams,
-                                    alignment_heads=self.settings.alignment_heads, weights=self._weights, dtype=self.engine_dtype)
+                                    alignment_heads=self.settings.alignment_heads, weights=self._weights, dtype=self.engine_dtype,
+                                    decoder_weights=self.decoder_weights)
         self._weights = self.engine.weights
         self._state_dict = None if self._weights is not None else self._state_dict
         self.capacity = capacity

@@ -58,7 +58,7 @@ class LocalWhisperBackend(TranscriptionBackend):
 
     def __init__(self, model, model_size: str = "S", chunk_length_s: int = 10, platform: str = "nvidia", torch_dtype=None,
                  language: str = "en", feature_extractor=None, tokenizer=None, revision: str = "main", asr_pipeline=None,
-                 batch_size: int = 1, device: str = "cuda"):
+                 batch_size: int = 1, device: str = "cuda", decoder_weights=None):
         if platform != "nvidia":
             raise ValueError(f"Invalid platform: {platform} (this build is the NVIDIA H100 engine)")
         self.chunk_length_s = chunk_length_s
@@ -70,7 +70,7 @@ class LocalWhisperBackend(TranscriptionBackend):
 
             asr_pipeline = ASRPipeline(model, model_size=model_size, chunk_length_s=chunk_length_s, torch_dtype=torch_dtype,
                                        device=device, feature_extractor=feature_extractor, tokenizer=tokenizer,
-                                       revision=revision, batch_size=batch_size)
+                                       revision=revision, batch_size=batch_size, decoder_weights=decoder_weights)
         self.asr_pipeline = asr_pipeline
 
     def _kwargs(self):
@@ -94,7 +94,7 @@ class StreamingPipeline:
                  backend: Optional[TranscriptionBackend] = None, use_remote_api: bool = False, api_url=None, api_auth_token=None,
                  api_model_name=None, api_lang_id=None, request_timeout_s=None, bytes_per_sample: int = 2,
                  sample_rate: int = 16000, revision="main", use_vad: bool = True, vad_threshold: float = 0.1,
-                 vad_no_speech_chunks: int = 1, vad_prepend_chunks: int = 3, vad_model=None):
+                 vad_no_speech_chunks: int = 1, vad_prepend_chunks: int = 3, vad_model=None, decoder_weights=None):
         self.sample_rate = sample_rate
         self.chunk_length_s = chunk_length_s
         self.min_process_chunk_s = min_process_chunk_s
@@ -107,7 +107,7 @@ class StreamingPipeline:
                 raise ValueError("model is required when using LocalWhisperBackend")
             backend = LocalWhisperBackend(model=model, model_size=model_size, chunk_length_s=chunk_length_s, platform=platform,
                                           torch_dtype=torch_dtype, language=language, feature_extractor=feature_extractor,
-                                          tokenizer=tokenizer, revision=revision)
+                                          tokenizer=tokenizer, revision=revision, decoder_weights=decoder_weights)
         self.backend = backend
         self.use_vad = use_vad
         self.vad_threshold = vad_threshold
