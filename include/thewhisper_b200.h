@@ -103,6 +103,13 @@ int bw_decode_begin(bw_engine* e, int32_t A, int32_t G, const int32_t* prompt_ho
 /* run n decoder steps (one CUDA-graph launch each, no host synchronisation).  Fails before launching anything when the
  * steps would run past position max_target_positions - 1 (counted from bw_decode_begin) */
 int bw_decode_run(bw_engine* e, int32_t n_steps, void* stream);
+/* Run the teacher-forced positions 0..n_positions-1 of every sequence begun by bw_decode_begin in one batched pass (or several,
+ * max_rows_per_pass = Q x positions per pass; 0 = engine default).  Afterwards the engine is in the state n_positions calls of
+ * bw_decode_run would have left it in, except that the logits buffer is not written.  Requires: called directly after
+ * bw_decode_begin, 1 <= n_positions <= begin_index - 1.  The first call allocates the scratch of one pass (a fixed budget of
+ * 4096 rows, or Q x max_target_positions when that is smaller: 178 MB at large-v3) and keeps it until bw_engine_destroy; every
+ * refusal, including a failed allocation, happens before anything is launched, so the engine stays as bw_decode_begin left it. */
+int bw_decode_prefill(bw_engine* e, int32_t n_positions, int32_t max_rows_per_pass, void* stream);
 /* kernels launched by bw_decode_run since the engine was created (kernel nodes of the step graph x graph launches);
  * bench.py reports it as part of "gpu_launches" */
 long long bw_decode_kernel_launches(bw_engine* e);

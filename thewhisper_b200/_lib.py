@@ -55,6 +55,7 @@ SYMBOLS = {
     "bw_encode": (C.c_int, [_P, _I, _P]),
     "bw_decode_begin": (C.c_int, [_P, _I, _I, _P, _I, C.POINTER(bw_decode_opts), _P]),
     "bw_decode_run": (C.c_int, [_P, _I, _P]),
+    "bw_decode_prefill": (C.c_int, [_P, _I, _I, _P]),
     "bw_decode_kernel_launches": (C.c_longlong, [_P]),
     "bw_decode_read": (C.c_int, [_P, _P, _P, _P, _P]),
     "bw_decode_reorder": (C.c_int, [_P, _P, _P, _P]),

@@ -23,8 +23,9 @@ def _topk_desc(values: np.ndarray, k: int) -> np.ndarray:
     return order[:, :k]
 
 
-def beam_search(eng, prompts: np.ndarray, A: int, G: int, opts, max_new: int, length_penalty: float = 1.0, return_beam_indices: bool = False):
-    """prompts [A, plen].  Returns (generated ids per audio (best beam, cut before EOS), n_steps, eos_seen) and, on request, the
+def beam_search(eng, prompts: np.ndarray, A: int, G: int, opts, max_new: int, length_penalty: float = 1.0, return_beam_indices: bool = False,
+                prefill: bool = False):
+    """prompts [A, plen] (prefill: teacher-forced positions in one batched prefill pass).  Returns (generated ids per audio (best beam, cut before EOS), n_steps, eos_seen) and, on request, the
     `beam_indices` of the returned sequences as GenerationMixin._beam_search keeps them (TF generation/utils.py:2984-2997,3065-3070):
     entry t = the global sequence slot (audio * G + beam) whose forward pass produced generated token t, -1 beyond the sequence."""
     plen = prompts.shape[1]
@@ -34,7 +35,10 @@ def beam_search(eng, prompts: np.ndarray, A: int, G: int, opts, max_new: int, le
     K = 2 * G
     rep = np.repeat(prompts, G, axis=0)
     eng.decode_begin(rep, A, G, opts)
-    eng.decode_run(plen - 1)  # teacher-forced prompt positions
+    if prefill and plen > 1:  # teacher-forced prompt positions
+        eng.decode_prefill(plen - 1)
+    else:
+        eng.decode_run(plen - 1)
 
     pad = opts.pad_token
     # (the bookkeeping arrays are as long as this decode can get, not max_target_positions: every step gathers and concatenates

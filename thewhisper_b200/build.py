@@ -16,7 +16,7 @@ OUT_DIR = os.path.join(HERE, "_C")
 LIB = os.path.join(OUT_DIR, "libthewhisper_b200.so")
 # compiled twice: 16-bit elements = bfloat16 (x.o) and, with -DBW_F16, = float16 (x_f16.o)
 SOURCES_PER_DTYPE = ["api.cu", "gemm_tc.cu", "gemm_dec.cu", "attn_enc.cu", "logmel.cu", "decode.cu", "decode_stream.cu",
-                     "decode_mega.cu", "timestamps.cu"]
+                     "decode_mega.cu", "decode_prefill.cu", "timestamps.cu"]
 SOURCES_ONCE = ["abi.cu", "hostproc.cu", "host_decode.cu"]
 HEADERS = ["common.cuh", "kernels.h", "decode.cuh", "decode_mega_common.cuh", "abi_rename.h", "abi_unrename.h",
            os.path.join("..", "..", "include", "thewhisper_b200.h")]

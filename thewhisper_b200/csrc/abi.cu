@@ -86,6 +86,9 @@ int bw_decode_begin(bw_engine* e, int32_t A, int32_t G, const int32_t* prompt, i
   BW_FWD(bw_decode_begin, e, A, G, prompt, plen, opts, stream);
 }
 int bw_decode_run(bw_engine* e, int32_t n_steps, void* stream) { BW_FWD(bw_decode_run, e, n_steps, stream); }
+int bw_decode_prefill(bw_engine* e, int32_t n_positions, int32_t max_rows_per_pass, void* stream) {
+  BW_FWD(bw_decode_prefill, e, n_positions, max_rows_per_pass, stream);
+}
 long long bw_decode_kernel_launches(bw_engine* e) {
   if (!e) return -1;
   return e->f16 ? bw_decode_kernel_launches_f16(BW_H(e)) : bw_decode_kernel_launches_bf16(BW_B(e));

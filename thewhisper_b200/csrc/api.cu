@@ -128,6 +128,11 @@ struct bw_engine {
   std::map<int, cudaGraphExec_t> enc_graphs;
   std::map<int, int> enc_calls;
   int num_sms = 132;
+  // prompt prefill (bw_decode_prefill): scratch of one pass of up to pf_rows rows, allocated by the first call
+  int pf_rows = 0;
+  long long pf_part_floats = 0;
+  float *pf_x = nullptr, *pf_part = nullptr;
+  bf16 *pf_n = nullptr, *pf_q = nullptr, *pf_a = nullptr, *pf_h = nullptr;
   unsigned* mega_bar = nullptr;
   long long* mega_trace = nullptr;
   std::map<std::string, std::pair<void*, size_t>> buffers;
@@ -335,6 +340,69 @@ int step_batched_impl(bw_engine* e, cudaStream_t st) {
   }
   return 0;
 }
+
+constexpr int PREFILL_ROWS = 4096;  // rows (sequence x position) of one prefill pass, unless the engine's Q * Tmax is smaller
+
+// One prefill pass: positions t0 .. t0 + n - 1 of all Q sequences as R = Q * n rows through the batched step's layer sequence (the
+// same gemm_dec projections at Q' = R, their split-K partial sums consumed by resid_ln / gelu_bias / the prefill kernels).  Only the
+// K / V cache rows are kept, so the last layer stops after its QKV projection and there is no final LayerNorm and no LM head.
+int prefill_pass(bw_engine* e, cudaStream_t st, int t0, int n) {
+  const int D = e->D, H = e->H, S = e->S, ffn = e->cfg.ffn, Tmax = e->Tmax, Q = e->Q, R = e->Q * n;
+  const long long self_layer = (long long)e->cfg.max_audios * e->cfg.max_beams * Tmax * D;
+  const long long cross_layer = (long long)e->cfg.max_audios * H * S * 64;
+  const bool w8 = e->embed_scale != nullptr;
+  auto proj = [&](const bf16* in, int K, const void* W, const float* sc, int N, int* ns) {
+    const DecGemmPlan pl = gemm_dec_plan(R, N, K, e->num_sms, true, w8);  // fits pf_part: prefill_fits checked it before any launch
+    GemmEpi ep;
+    ep.out_f32 = e->pf_part; ep.row_stride = N;
+    *ns = pl.ksplit;
+    return gemm_dec(st, in, W, sc, R, N, K, 0, ep, pl, (long long)R * N);
+  };
+  if (int rc = launch_prefill_embed(st, e->embed, e->embed_scale, e->dec_pos, e->tokens, e->pf_x, Q, n, t0, D, Tmax)) return rc;
+  int ns = 0;
+  const float* pbias = nullptr;
+  for (size_t l = 0; l < e->dec.size(); ++l) {
+    const DecLayer& L = e->dec[l];
+    bf16* kc = e->self_k + l * self_layer;
+    bf16* vc = e->self_v + l * self_layer;
+    const bool last = l + 1 == e->dec.size();
+    if (int rc = launch_resid_ln(st, e->pf_x, e->pf_part, ns, (long long)R * D, pbias, L.ln1g, L.ln1b, e->pf_n, R, D)) return rc;
+    if (int rc = proj(e->pf_n, D, L.wqkv, L.sc[0], 3 * D, &ns)) return rc;
+    if (int rc = launch_prefill_proj_sum(st, e->pf_part, ns, (long long)R * 3 * D, L.bqkv, 3 * D, D, R, last ? nullptr : e->pf_q, kc, vc, n,
+                                         t0, Tmax))
+      return rc;
+    if (last) break;
+    if (int rc = launch_prefill_self_attn(st, e->pf_q, kc, vc, e->pf_a, Q, n, t0, H, Tmax)) return rc;
+    if (int rc = proj(e->pf_a, D, L.wo, L.sc[1], D, &ns)) return rc;
+    if (int rc = launch_resid_ln(st, e->pf_x, e->pf_part, ns, (long long)R * D, L.bo, L.ln2g, L.ln2b, e->pf_n, R, D)) return rc;
+    if (int rc = proj(e->pf_n, D, L.xwq, L.sc[2], D, &ns)) return rc;
+    if (int rc = launch_prefill_proj_sum(st, e->pf_part, ns, (long long)R * D, L.xbq, D, D, R, e->pf_q, nullptr, nullptr, n, t0, Tmax)) return rc;
+    if (int rc = launch_prefill_cross_attn(st, e->pf_q, e->cross_k + l * cross_layer, e->cross_v + l * cross_layer, e->pf_a, e->A, e->G, n, S, H))
+      return rc;
+    if (int rc = proj(e->pf_a, D, L.xwo, L.sc[3], D, &ns)) return rc;
+    if (int rc = launch_resid_ln(st, e->pf_x, e->pf_part, ns, (long long)R * D, L.xbo, L.ln3g, L.ln3b, e->pf_n, R, D)) return rc;
+    if (int rc = proj(e->pf_n, D, L.w1, L.sc[4], ffn, &ns)) return rc;
+    if (int rc = launch_gelu_bias(st, e->pf_part, ns, (long long)R * ffn, L.b1, e->pf_h, R, ffn)) return rc;
+    if (int rc = proj(e->pf_h, ffn, L.w2, L.sc[5], D, &ns)) return rc;
+    pbias = L.b2;
+  }
+  return 0;
+}
+
+// every projection of a pass of R rows keeps its split-K partial sums within pf_part (checked before anything is launched, so a
+// refused prefill leaves the cache untouched)
+int prefill_fits(bw_engine* e, int R) {
+  const int D = e->D, ffn = e->cfg.ffn;
+  const int nk[4][2] = {{3 * D, D}, {D, D}, {ffn, D}, {D, ffn}};
+  for (const auto& p : nk) {
+    const DecGemmPlan pl = gemm_dec_plan(R, p[0], p[1], e->num_sms, true, e->embed_scale != nullptr);
+    BW_CHECK((long long)pl.ksplit * R * p[0] <= e->pf_part_floats, "bw_decode_prefill: %d splits x %d rows x N=%d exceed the partial-sum buffer",
+             pl.ksplit, R, p[0]);
+  }
+  return 0;
+}
+
+__global__ void set_pos_kernel(int* pos, int v) { *pos = v; }
 
 // one decoder step for all Q sequences (enqueued on st; captured into a CUDA graph by the caller)
 int step_impl(bw_engine* e, cudaStream_t st) {
@@ -924,6 +992,50 @@ int bw_decode_run(bw_engine* e, int32_t n_steps, void* stream) {
       if (int rc = step_impl(e, st)) return rc;
     }
   }
+  return 0;
+}
+
+int bw_decode_prefill(bw_engine* e, int32_t n_positions, int32_t max_rows_per_pass, void* stream) {
+  BW_CHECK(e && e->finalized && e->Q > 0, "bw_decode_prefill: no decode in progress");
+  BW_CHECK(e->steps == 0, "bw_decode_prefill: %d decoder steps have run since bw_decode_begin; the prefill must come first", e->steps);
+  BW_CHECK(n_positions >= 1 && n_positions <= e->opts.begin_index - 1, "bw_decode_prefill: n_positions=%d outside 1..begin_index-1 = 1..%d",
+           n_positions, e->opts.begin_index - 1);
+  BW_CHECK(max_rows_per_pass == 0 || max_rows_per_pass >= e->Q, "bw_decode_prefill: max_rows_per_pass=%d is below the %d sequences of one position",
+           max_rows_per_pass, e->Q);
+  const bw_config& c = e->cfg;
+  if (!e->pf_h) {  // (pf_h is allocated last: a call after a failed allocation starts over)
+    const long long qm = (long long)c.max_audios * c.max_beams;
+    e->pf_rows = (int)(qm * e->Tmax < PREFILL_ROWS ? qm * e->Tmax : (qm > PREFILL_ROWS ? qm : PREFILL_ROWS));
+    const size_t rows = (size_t)e->pf_rows;
+    const int widest = c.ffn > 3 * e->D ? c.ffn : 3 * e->D;
+    // split-K partial sums: ksplit = 1 holds R x N floats; ksplit > 1 only when ksplit x (CTAs of one split) <= SMs, i.e. at most
+    // SMs x (128 weight rows x 256 sequence rows) floats
+    e->pf_part_floats = (long long)rows * widest > (long long)e->num_sms * 128 * 256 ? (long long)rows * widest : (long long)e->num_sms * 128 * 256;
+    const char* names[5] = {"pf_x", "pf_part", "pf_n", "pf_q", "pf_a"};
+    for (const char* nm : names) {  // free what an earlier, failed call allocated
+      auto it = e->buffers.find(nm);
+      if (it != e->buffers.end()) {
+        cudaFree(it->second.first);
+        e->buffers.erase(it);
+      }
+    }
+    if (dalloc(e, "pf_x", &e->pf_x, rows * e->D, false) || dalloc(e, "pf_part", &e->pf_part, (size_t)e->pf_part_floats, false) ||
+        dalloc(e, "pf_n", &e->pf_n, rows * e->D, false) || dalloc(e, "pf_q", &e->pf_q, rows * e->D, false) ||
+        dalloc(e, "pf_a", &e->pf_a, rows * e->D, false) || dalloc(e, "pf_h", &e->pf_h, rows * c.ffn, false))
+      return -1;
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int rows = (max_rows_per_pass > 0 && max_rows_per_pass < e->pf_rows) ? max_rows_per_pass : e->pf_rows;
+  const int per = rows / e->Q;
+  for (int t0 = 0; t0 < n_positions; t0 += per)
+    if (int rc = prefill_fits(e, e->Q * (n_positions - t0 < per ? n_positions - t0 : per))) return rc;
+  for (int t0 = 0; t0 < n_positions; t0 += per) {
+    const int n = n_positions - t0 < per ? n_positions - t0 : per;
+    if (int rc = prefill_pass(e, st, t0, n)) return rc;
+  }
+  set_pos_kernel<<<1, 1, 0, st>>>(e->pos, n_positions);
+  BW_CUDA_OK(cudaGetLastError());
+  e->steps = n_positions;
   return 0;
 }
 

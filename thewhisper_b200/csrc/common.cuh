@@ -348,6 +348,9 @@ int make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_
 // the same for a 2-D uint8 tensor (int8 weight codes), unswizzled: box_cols bytes per row
 int make_tmap_2d_u8(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t row_pitch_bytes, uint32_t box_rows,
                     uint32_t box_cols);
+// 3-D: batch x rows x cols, both pitches in bytes; coordinates past rows (or batch) read as zeros
+int make_tmap_3d_bf16(CUtensorMap* out, const void* base, uint64_t batch, uint64_t rows, uint64_t cols, uint64_t row_pitch_bytes,
+                      uint64_t batch_pitch_bytes, uint32_t box_rows, uint32_t box_cols);
 // multiprocessor count of the current device (queried once)
 int device_sms();
 

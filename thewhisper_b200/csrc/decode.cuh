@@ -162,4 +162,18 @@ int launch_select(cudaStream_t st, const SelectArgs& a);
 int launch_resid_ln(cudaStream_t st, float* x, const float* part, int nsplit, long long split_stride, const float* bias, const float* g,
                     const float* b, bf16* y, int Q, int D);
 
+
+// ---- prompt prefill (decode_prefill.cu): R = Q * n rows, row r = q * n + i is sequence q at position t0 + i ----
+// x[r] = E[token[q, t]] (* Es[token] for int8 rows) + P[t]
+int launch_prefill_embed(cudaStream_t st, const void* E, const float* Es, const float* P, const int* tokens, float* x, int Q, int n, int t0,
+                         int D, int Tmax);
+// split-K partial sums [nsplit][R][N] (+ bias) -> q / 8 as 16-bit rows [R][D] (qout may be null); N = 3D also appends the rows' K / V
+// to the cache kc / vc [Q][Tmax][D]
+int launch_prefill_proj_sum(cudaStream_t st, const float* part, int nsplit, long long split_stride, const float* bias, int N, int D, int R,
+                            bf16* qout, bf16* kc, bf16* vc, int n, int t0, int Tmax);
+// causal self-attention of the pass's rows over cache rows [0, t0 + i] of their sequence -> out [R][D]
+int launch_prefill_self_attn(cudaStream_t st, const bf16* q, const bf16* kc, const bf16* vc, bf16* out, int Q, int n, int t0, int H, int Tmax);
+// cross-attention: the G * n rows of audio a over its S encoder positions (kc / vc [A][H][S][64]) -> out [R][D]
+int launch_prefill_cross_attn(cudaStream_t st, const bf16* q, const bf16* kc, const bf16* vc, bf16* out, int A, int G, int n, int S, int H);
+
 }  // namespace bw

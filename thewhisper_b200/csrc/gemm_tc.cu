@@ -293,8 +293,8 @@ int make_tmap_2d_u8(CUtensorMap* out, const void* base, uint64_t rows, uint64_t 
   return 0;
 }
 
-static int make_tmap_3d_bf16(CUtensorMap* out, const void* base, uint64_t batch, uint64_t rows, uint64_t cols,
-                             uint64_t row_pitch_bytes, uint64_t batch_pitch_bytes, uint32_t box_rows, uint32_t box_cols) {
+int make_tmap_3d_bf16(CUtensorMap* out, const void* base, uint64_t batch, uint64_t rows, uint64_t cols,
+                      uint64_t row_pitch_bytes, uint64_t batch_pitch_bytes, uint32_t box_rows, uint32_t box_cols) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return -1;
   cuuint64_t dims[3] = {cols, rows, batch};

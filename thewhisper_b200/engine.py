@@ -334,6 +334,12 @@ class WhisperEngine:
         self.stats["decode_steps"] += n_steps
         self.stats["sequence_steps"] += n_steps * self._Q
 
+    def decode_prefill(self, n_positions: int, max_rows_per_pass: int = 0) -> None:
+        """Run the teacher-forced positions 0..n_positions-1 of every sequence in one batched pass (or several of at most
+        max_rows_per_pass = sequences x positions rows; 0 = the engine's default): the state n_positions decode_run steps
+        leave, except the logits.  Must directly follow decode_begin; n_positions <= begin_index - 1."""
+        _lib.check(self.lib.bw_decode_prefill(self.h, n_positions, max_rows_per_pass, self._stream()))
+
     def decode_kernel_launches(self) -> int:
         """Kernels launched by decode_run so far (counted from the captured step graphs)."""
         return int(self.lib.bw_decode_kernel_launches(self.h))
@@ -369,14 +375,19 @@ class WhisperEngine:
         vp = (self.dims.vocab + 31) // 32 * 32  # row pitch of the engine's logits buffer (rows stay 16-byte aligned)
         return self.buffer("logits", torch.float32, (self.max_audios * self.max_beams, vp))[: self._Q, : self.dims.vocab]
 
-    def greedy(self, prompts: np.ndarray, A: int, opts: DecodeOptions, max_new_tokens: int, poll_every: int = 32):
+    def greedy(self, prompts: np.ndarray, A: int, opts: DecodeOptions, max_new_tokens: int, poll_every: int = 32,
+               prefill: bool = False):
         """Greedy decode of A audios (their cross K/V must be resident from encode()).  Returns generated ids per
-        audio (prompt stripped, cut at and excluding EOS) and the raw token matrix."""
+        audio (prompt stripped, cut at and excluding EOS) and the raw token matrix.  prefill: run the teacher-forced
+        positions as one batched prefill pass instead of step by step."""
         plen = prompts.shape[1]
         Tmax = self.dims.max_target_positions
         max_new = max(0, min(max_new_tokens, Tmax - plen))
         self.decode_begin(prompts, A, 1, opts)
-        self.decode_run(plen - 1)  # teacher-forced prompt positions 0..plen-2
+        if prefill and plen > 1:  # teacher-forced prompt positions 0..plen-2
+            self.decode_prefill(plen - 1)
+        else:
+            self.decode_run(plen - 1)
         done = 0
         toks = fin = None
         while done < max_new:

@@ -137,17 +137,19 @@ class WhisperGenerator:
         return np.asarray(rows, dtype=np.int32)
 
     # --------------------------------------------------------------------------------------------------------
-    def _decode(self, prompts: np.ndarray, A: int, opts: DecodeOptions, max_new: int, num_beams: int):
-        """-> (list of generated id arrays cut before EOS, n_steps HF would have run, eos_seen per row)"""
+    def _decode(self, prompts: np.ndarray, A: int, opts: DecodeOptions, max_new: int, num_beams: int, prefill: bool = False):
+        """-> (list of generated id arrays cut before EOS, n_steps HF would have run, eos_seen per row).  prefill: the
+        teacher-forced positions run as one batched prefill pass (a prompt), not step by step."""
         self._beam_indices = None
+        kw = {"prefill": True} if prefill else {}
         if num_beams > 1:
             from .beam import beam_search
 
             if opts.record_alignment:  # token timestamps need to know which slot produced each token of the winner
-                gen, steps, eos_seen, self._beam_indices = beam_search(self.eng, prompts, A, num_beams, opts, max_new, return_beam_indices=True)
+                gen, steps, eos_seen, self._beam_indices = beam_search(self.eng, prompts, A, num_beams, opts, max_new, return_beam_indices=True, **kw)
                 return gen, steps, eos_seen
-            return beam_search(self.eng, prompts, A, num_beams, opts, max_new)
-        gen, toks, done = self.eng.greedy(prompts, A, opts, max_new)
+            return beam_search(self.eng, prompts, A, num_beams, opts, max_new, **kw)
+        gen, toks, done = self.eng.greedy(prompts, A, opts, max_new, **kw)
         plen = prompts.shape[1]
         first_eos = []
         for a in range(A):
@@ -232,11 +234,24 @@ class WhisperGenerator:
     def generate(self, B: int, num_frames: Optional[np.ndarray] = None, mel_f32: Optional[torch.Tensor] = None,
                  return_timestamps: bool = False, return_token_timestamps: bool = False, language=None, task=None,
                  num_beams: int = 1, max_new_tokens: Optional[int] = None, extra_suppress: Sequence[int] = (),
-                 encoded: bool = False):
+                 encoded: bool = False, prompt_ids=None, prompt_condition_type: Optional[str] = None):
         """The engine's mel buffer must hold the B chunks (engine.logmel / set_mel).  Returns a dict with
         "sequences" (list of int arrays: generated ids, prompt and EOS stripped), optionally "token_timestamps"
-        (list of float arrays aligned with sequences) and "segments"."""
+        (list of float arrays aligned with sequences) and "segments".
+        prompt_ids (tensor, array or list of ids, e.g. from get_prompt_ids): decoded as prompt + init tokens on every window, as
+        transformers' short-form generate does (generation_whisper.py _prepare_decoder_input_ids); the prompt positions run through
+        the decoder in one batched prefill pass."""
         eng, st = self.eng, self.st
+        if prompt_condition_type not in (None, "first-segment", "all-segments"):
+            raise ValueError(f"`prompt_condition_type={prompt_condition_type} does not exist. Make sure to set `prompt_condition_type` "
+                             "to one of first-segment, all-segments")
+        if prompt_condition_type == "all-segments":
+            raise NotImplementedError("prompt_condition_type='all-segments' needs condition_on_prev_tokens, which the engine does not implement")
+        prompt = None
+        if prompt_ids is not None:
+            if isinstance(prompt_ids, torch.Tensor):
+                prompt_ids = prompt_ids.detach().cpu().numpy()
+            prompt = np.asarray(prompt_ids, dtype=np.int64).reshape(-1).astype(np.int32)
         F = eng.frames
         if return_token_timestamps:
             return_timestamps = True
@@ -250,9 +265,16 @@ class WhisperGenerator:
         if not encoded:
             eng.encode(B)
         prompts_all = self.init_tokens(B, language, task, return_timestamps)
+        if prompt is not None:  # decoder input = prompt + init tokens; begin_index, the length checks and timestamps count all of it
+            prompts_all = np.concatenate([np.repeat(prompt[None, :], B, axis=0), prompts_all], axis=1)
         plen = prompts_all.shape[1]
-        max_new = max_new_tokens if max_new_tokens is not None else st.max_length - plen
         mtp = eng.dims.max_target_positions
+        if max_new_tokens is not None:
+            max_new = max_new_tokens
+        elif prompt is not None:  # _set_max_new_tokens_and_length: max_length grows by the conditioning tokens, up to max_target_positions
+            max_new = min(st.max_length + min(mtp // 2 - 1, plen - 1), mtp) - plen
+        else:
+            max_new = st.max_length - plen
         if (max_new_tokens or 0) + plen > mtp:  # same check, same message as TF generation_whisper.py:1920-1930
             raise ValueError(
                 f"The length of `decoder_input_ids`, including special start tokens, prompt tokens, and previous tokens, is {plen}, "
@@ -283,7 +305,7 @@ class WhisperGenerator:
                 eng.encode(A)
             first = False
             prompts = prompts_all[rows]
-            gen, n_steps, _ = self._decode(prompts, A, opts, max_new, num_beams)
+            gen, n_steps, _ = self._decode(prompts, A, opts, max_new, num_beams, **({"prefill": True} if prompt is not None else {}))
             tts = None
             if return_token_timestamps:
                 tts = self._token_timestamps(A, plen, n_steps, (num_frames - seek)[rows])

@@ -207,7 +207,8 @@ class ASRPipeline:
             out = self.generator.generate(
                 B, num_frames=num_frames, mel_f32=mel, return_timestamps=bool(return_timestamps),
                 return_token_timestamps=(return_timestamps == "word"), language=generate_kwargs.get("language"),
-                task=generate_kwargs.get("task"), num_beams=num_beams, max_new_tokens=generate_kwargs.get("max_new_tokens"))
+                task=generate_kwargs.get("task"), num_beams=num_beams, max_new_tokens=generate_kwargs.get("max_new_tokens"),
+                prompt_ids=generate_kwargs.get("prompt_ids"), prompt_condition_type=generate_kwargs.get("prompt_condition_type"))
             for j, g in enumerate(group):
                 o: Dict[str, Any] = {"tokens": np.asarray(out["sequences"][j], dtype=np.int64)[None, :]}
                 if return_timestamps == "word":
