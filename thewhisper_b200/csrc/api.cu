@@ -427,7 +427,7 @@ int step_impl(bw_engine* e, cudaStream_t st) {
     m.embed = e->embed; m.embed_scale = e->embed_scale; m.wscale = e->wscale_tab; m.dec_pos = e->dec_pos; m.lnf_g = e->dec_lnf_g; m.lnf_b = e->dec_lnf_b;
     m.tokens = e->tokens; m.pos = e->pos; m.ldl = e->Vp;
     m.dx = e->dx; m.dqkv = e->dqkv; m.dattn = e->dattn; m.dq = e->dq; m.dh = e->dh; m.logits = e->logits;
-    m.part_o = e->part_o; m.part_ml = e->part_ml; m.xcounters = e->xcounters; m.bar = e->mega_bar;
+    m.part_o = e->part_o; m.part_ml = e->part_ml; m.bar = e->mega_bar;
     int ns = e->num_sms / (Q * H);
     const int ns_min = (S + 255) / 256;
     if (ns < ns_min) ns = ns_min;

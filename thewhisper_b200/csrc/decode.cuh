@@ -120,7 +120,6 @@ struct MegaArgs {
   const int* pos;
   float *dx, *dqkv, *dattn, *dq, *dh, *logits;
   float *part_o, *part_ml;  // cross-attention partials [Q][H][nsplit][64], [..][2]
-  unsigned* xcounters;      // [Q*H]
   unsigned* bar;
   int nsplit;
   // alignment (word timestamps)

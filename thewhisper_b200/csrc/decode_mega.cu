@@ -32,7 +32,14 @@
 //     into the second slab region, reads DRAM itself: the cross-q barrier falls to 1.0 us and the step from 1.19-1.20 to
 //     1.13-1.16 ms (H100 80GB HBM3, 400 W power limit).  Only the cross-attention K/V, read by a bulk load three phases
 //     later, are still prefetched: without that the cross-attention phase took 6.7 us instead of 5.9 us (the step times of the
-//     two were within each other's spread).
+//     two were within each other's spread);
+//   * the cross-attention key splits are merged by their consumer: each CTA's cross out-projection staging reads the partials
+//     of every split (merge_xattn, one round of independent L2 loads).  When the last-arriving split of each head merged them in
+//     phase E, behind an acq_rel counter and a second dependent round trip, every CTA waited for that at the barrier.  The DMA
+//     warp queues the fc1 slab copy (~100 KB per SM) only once the merge loads are issued: queued first, it held them back.
+//     H100 80GB HBM3 at 700 W, bench.py: 849-850 tok/s instead of 812-814 (829-830 with the copy queued first).  The traced
+//     instantiation does not show it: E's work falls from 5.9-6.2 to 4.5 us, but F's rises from 1.7 to 4.1 us and fc2's
+//     x staging from 0.6 to 3.4 us, and its step span is not shorter -- take step times from the untraced kernel.
 // After a barrier only the x row (and the residual values of the rows a warp owns) have to be fetched.
 //
 // Work split: 12 warps per CTA, global warp id gw; a GEMV phase gives warp gw the R rows starting at gw*R (one pass:
@@ -160,7 +167,7 @@ __device__ __forceinline__ GemvDesc make_desc(const MegaArgs& a, const MegaLayer
       d.W = static_cast<const uint8_t*>(L.xwq); d.bias = L.xbq; d.src = a.dx; d.lng = L.ln2g; d.lnb = L.ln2b; d.out = a.dq; d.alpha = 0.125f; d.alpha_cols = a.D;
       break;
     case 3:
-      d.W = static_cast<const uint8_t*>(L.xwo); d.bias = L.xbo; d.src = a.dattn; d.out = a.dx; d.residual = a.dx;
+      d.W = static_cast<const uint8_t*>(L.xwo); d.bias = L.xbo; d.src = a.part_o; d.out = a.dx; d.residual = a.dx;  // x: merge_xattn
       break;
     case 4:
       d.W = static_cast<const uint8_t*>(L.w1); d.bias = L.b1; d.N = a.ffn; d.src = a.dx; d.lng = L.ln3g; d.lnb = L.ln3b; d.out = a.dh; d.ldo = a.ffn; d.act = 1;
@@ -218,7 +225,80 @@ __device__ __forceinline__ void prefetch_phase(const GemvDesc& d, Pre& p, uint8_
   }
 }
 
-// stage M rows of K floats into smem (ld.global.cg), LayerNormed when the phase has one.
+// The cross out-projection's x: the cross-attention output of each sequence, merged here from the partials of its nsplit key
+// splits (part_o [Q][H][nsplit][64], part_ml [..][2] = (max, sum)) that phase E left, so that phase E ends at its barrier arrival.
+// Thread t stages elements [4t, 4t + 4) of a sequence: lane j of a 16-lane group (one head) reads split j's (max, sum) and the
+// group shares them by shuffle; the loads of the first XC splits are issued before any is used, so for nsplit <= XC a
+// sequence costs one round of L2 reads, queued before the DMA warp's slab copy of the next phase.  (At Q = 2 the sequences go
+// one after the other: both rounds in flight together would need ~50 more registers than the kernel's peak.)  The arithmetic (the pl > 0 predicate, the maximum, __expf weights,
+// fmaf sums in split order, one division) is fixed, so every CTA stages the same x bit for bit.  The CTA also stores its own
+// rows [n0, nend) of x to dattn: nothing in the step reads them, but after the step dattn holds the last layer's
+// cross-attention output as on the other step paths.
+template <int MB>
+__device__ __forceinline__ void merge_xattn(float* xs, const GemvDesc& d, const MegaArgs& a, int M) {
+  constexpr int XC = 6;  // splits per round of loads (large-v3 on 132 SMs: nsplit = 6)
+  static_assert(MAXD <= (MT - 32) * 4 && XSPLIT <= 16, "one float4 per staging thread and sequence; one lane per split");
+  const int K = d.K, nsplit = a.nsplit;
+  const int k = threadIdx.x * 4, sp_l = threadIdx.x & 15;
+  const bool have = k < K;
+#pragma unroll 1
+  for (int m = 0; m < MB; ++m) {
+    const int hb = (m * a.H + (k >> 6)) * nsplit;  // (sequence, head) of this thread's elements
+    const float* po_base = a.part_o + hb * 64 + (k & 63);
+    const bool live = have && m < M;
+    float pm = -INFINITY, pl = 0.f;
+    float4 po[XC];
+    if (live && sp_l < nsplit) {
+      const float2 v = __ldcg(reinterpret_cast<const float2*>(a.part_ml) + hb + sp_l);
+      pm = v.x;
+      pl = v.y;
+    }
+#pragma unroll
+    for (int sp = 0; sp < XC; ++sp) {
+      po[sp] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (live && sp < nsplit) po[sp] = __ldcg(reinterpret_cast<const float4*>(po_base + sp * 64));
+    }
+    if (m == 0) asm volatile("bar.arrive 2, %0;" ::"n"(MT) : "memory");  // loads issued: the DMA warp may queue its copies
+    float mx = pl > 0.f ? pm : -INFINITY;  // fmaxf is exact: the tree gives the split-order maximum
+#pragma unroll
+    for (int s = 8; s >= 1; s >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, s));
+    float lsum = 0.f;
+    float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int sp0 = 0;;) {
+#pragma unroll
+      for (int sp = 0; sp < XC; ++sp) {
+        const float sm = __shfl_sync(0xffffffffu, pm, sp0 + sp, 16), sl = __shfl_sync(0xffffffffu, pl, sp0 + sp, 16);
+        if (sp0 + sp < nsplit && sl > 0.f) {
+          const float w = __expf(sm - mx);
+          lsum = fmaf(sl, w, lsum);
+          o.x = fmaf(po[sp].x, w, o.x);
+          o.y = fmaf(po[sp].y, w, o.y);
+          o.z = fmaf(po[sp].z, w, o.z);
+          o.w = fmaf(po[sp].w, w, o.w);
+        }
+      }
+      sp0 += XC;
+      if (sp0 >= nsplit) break;
+#pragma unroll
+      for (int sp = 0; sp < XC; ++sp)
+        if (live && sp0 + sp < nsplit) po[sp] = __ldcg(reinterpret_cast<const float4*>(po_base + (sp0 + sp) * 64));
+    }
+    if (!have) continue;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (m < M) {
+      v = make_float4(o.x / lsum, o.y / lsum, o.z / lsum, o.w / lsum);
+      float* row = a.dattn + m * K;
+      if (k >= d.n0 && k < d.nend) row[k] = v.x;
+      if (k + 1 >= d.n0 && k + 1 < d.nend) row[k + 1] = v.y;
+      if (k + 2 >= d.n0 && k + 2 < d.nend) row[k + 2] = v.z;
+      if (k + 3 >= d.n0 && k + 3 < d.nend) row[k + 3] = v.w;
+    }
+    *reinterpret_cast<float4*>(xs + m * K + k) = v;
+  }
+}
+
+// stage M rows of K floats into smem (ld.global.cg), LayerNormed when the phase has one; xattn (the cross out-projection):
+// x is merged from the cross-attention partials instead (merge_xattn).
 // The last warp takes no part in the staging: it runs `dma` (the TMA requests of the coming phases, ~0.25 us of issue
 // time) meanwhile and only joins the final CTA barrier.  The staging warps synchronise among themselves on named barrier 1.
 __device__ __forceinline__ void stage_sync() { asm volatile("bar.sync 1, %0;" ::"n"(MT - 32) : "memory"); }
@@ -233,12 +313,20 @@ __device__ __forceinline__ void stage_done_stagers() {
 __device__ __forceinline__ void stage_done_dma() { asm volatile("bar.sync 3, %0;" ::"n"(MT) : "memory"); }
 
 template <int MB, unsigned VAR, class Dma>
-__device__ __forceinline__ void stage_x(float* xs, float* red, const GemvDesc& d, const Pre& p, int M, bool split_end, Dma&& dma) {
+__device__ __forceinline__ void stage_x(float* xs, float* red, const GemvDesc& d, const Pre& p, int M, bool split_end, const MegaArgs& a,
+                                        bool xattn, Dma&& dma) {
   const int K = d.K;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == MW - 1) {
+    if (xattn) asm volatile("bar.sync 2, %0;" ::"n"(MT) : "memory");  // after the merge loads (merge_xattn)
     dma();
     if (split_end) stage_done_dma();
+    else __syncthreads();
+    return;
+  }
+  if (xattn) {
+    merge_xattn<MB>(xs, d, a, M);
+    if (split_end) stage_done_stagers();
     else __syncthreads();
     return;
   }
@@ -353,7 +441,6 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
   float* xs = red + 64;
   uint8_t* pool = reinterpret_cast<uint8_t*>(xs + (size_t)MB * a.ffn);
   uint8_t* att = pool + ATT_OFF;  // only R=1 slabs (<= 30 KB) are live while an attention phase runs
-  __shared__ unsigned s_last;
   __shared__ __align__(8) uint64_t wbar[2 * MW];  // per warp: slab barrier (+ second stage for the LM head)
   __shared__ __align__(8) uint64_t xbar;          // cross-attention K/V item
   __shared__ __align__(8) uint64_t cbar[2];       // the CTA's weight slabs of a layer phase (one per slab region)
@@ -449,7 +536,7 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
           }
         }
       };
-      stage_x<MB, VAR>(xs, red, cur, pre, Q, split_end, ahead);
+      stage_x<MB, VAR>(xs, red, cur, pre, Q, split_end, a, g == 3, ahead);
       mark(2);
       if (mkbase && lane == 0) wts[warp][0] = wts[warp][1] = 0;
       if (active) {
@@ -542,7 +629,7 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
         }
       }
       bar.wait();
-      // ---------------- E: cross-attention, (audio, head, key split) items; last split of a head merges ----------------
+      // ---------------- E: cross-attention, (audio, head, key split) items; phase F merges the splits ----------------
       {
         uint8_t* sK = att;
         uint8_t* sV = att + XKMAX * 128;
@@ -579,47 +666,12 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
           float mx, sum, ov;
           attend_smem<(XKMAX + KG - 1) / KG>(sK, sV, redo, red, qv, n, align_row, mx, sum, ov,
                                              (mkbase && bar.epoch < MEGA_TRACE_N) ? mkbase + bar.epoch * 4 : nullptr);
+          // the split's partials: every CTA's cross out-projection staging merges them after the barrier (merge_xattn)
           const long long pb = ((long long)q * H + h) * nsplit + split;
           if (threadIdx.x < 64) a.part_o[pb * 64 + threadIdx.x] = ov;
           if (threadIdx.x == 0) {
             a.part_ml[pb * 2 + 0] = mx;
             a.part_ml[pb * 2 + 1] = sum;
-          }
-          // merge by the last-arriving split of this (sequence, head): the partial stores above happen-before thread 0's
-          // acq_rel atomic through the CTA barrier; the last arriver's acquire makes every split's partials visible
-          __syncthreads();
-          if (threadIdx.x == 0) {
-            const unsigned prev = atom_acq_rel_add(&a.xcounters[q * H + h], 1u);
-            s_last = (prev == (unsigned)(nsplit - 1)) ? 1u : 0u;
-          }
-          __syncthreads();
-          if (s_last && threadIdx.x < 64) {
-            const long long hb = ((long long)q * H + h) * nsplit;
-            float pm[XSPLIT], pl[XSPLIT], po[XSPLIT];
-#pragma unroll
-            for (int sp = 0; sp < XSPLIT; ++sp) {
-              pm[sp] = -INFINITY; pl[sp] = 0.f; po[sp] = 0.f;
-              if (sp < nsplit) {
-                pm[sp] = __ldcg(&a.part_ml[(hb + sp) * 2]);
-                pl[sp] = __ldcg(&a.part_ml[(hb + sp) * 2 + 1]);
-                po[sp] = __ldcg(&a.part_o[(hb + sp) * 64 + threadIdx.x]);
-              }
-            }
-            float M = -INFINITY;
-#pragma unroll
-            for (int sp = 0; sp < XSPLIT; ++sp)
-              if (pl[sp] > 0.f) M = fmaxf(M, pm[sp]);
-            float Lsum = 0.f, o = 0.f;
-#pragma unroll
-            for (int sp = 0; sp < XSPLIT; ++sp) {
-              if (pl[sp] > 0.f) {
-                const float w = __expf(pm[sp] - M);
-                Lsum = fmaf(pl[sp], w, Lsum);
-                o = fmaf(po[sp], w, o);
-              }
-            }
-            a.dattn[(long long)q * D + h * 64 + threadIdx.x] = o / Lsum;
-            if (threadIdx.x == 0) a.xcounters[q * H + h] = 0u;
           }
           fence_proxy_async_smem();
           __syncthreads();
@@ -632,7 +684,7 @@ __global__ void __launch_bounds__(MT, 1) decode_mega_kernel(const __grid_constan
   }
 
   // ---------------- final LayerNorm + tied LM head: row pairs, two slab stages per warp ----------------
-  stage_x<MB, VAR>(xs, red, cur, pre, Q, split_end, [] {});
+  stage_x<MB, VAR>(xs, red, cur, pre, Q, split_end, a, false, [] {});
   unsigned long long best = 0ull;  // of the logits this lane finished: (order-preserving value bits << 32) | ~token
   {
     const int K = cur.K, N = cur.N;

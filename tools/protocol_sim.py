@@ -285,24 +285,28 @@ def mega1_programs(G, D, H, ffn, nsplit, L, p2p=False, prod=False):
                     p.append(("signal", ("xq", h)))
             else:
                 p.append(("barrier",))
-            # E: cross-attention, (head, split) items; the last-arriving split of a head merges
+            # E: cross-attention, (head, split) items.  Shipped: every split only writes its partials, and every CTA merges all
+            # of them while staging F (writing its own rows of dattn); V_PROD: the last-arriving split of a head merges
             if b < H * nsplit:
                 h, j = b // nsplit, b % nsplit
                 if p2p:
                     p.append(("wait", ("xq", h), (l + 1) * expected(h, D, 1, (D + G - 1) // G)))
                 p.append(("r", "dq", [h * 64 + d for d in range(64)], f"xq@{l}"))
                 p.append(("w", "part", [(h, j)], f"part@{l}"))
-                tail = [("r", "part", [(h, jj) for jj in range(nsplit)], f"part@{l}"),
-                        ("w", "dattn", range(h * 64, h * 64 + 64), f"a2@{l}")]
                 if prod:
-                    tail.append(("signal", ("prodE",)))
-                p.append(("merge", ("xc", h), (l + 1) * nsplit, tail))
+                    tail = [("r", "part", [(h, jj) for jj in range(nsplit)], f"part@{l}"),
+                            ("w", "dattn", range(h * 64, h * 64 + 64), f"a2@{l}"), ("signal", ("prodE",))]
+                    p.append(("merge", ("xc", h), (l + 1) * nsplit, tail))
             if prod:
                 p.append(("wait", ("prodE",), (l + 1) * H))
             else:
                 p.append(("barrier",))
             # F: cross out-proj + residual
-            p.append(("r", "dattn", allD, f"a2@{l}"))
+            if prod:
+                p.append(("r", "dattn", allD, f"a2@{l}"))
+            else:
+                p.append(("r", "part", [(h, jj) for h in range(H) for jj in range(nsplit)], f"part@{l}"))
+                p.append(("w", "dattn", rd, f"a2@{l}"))
             p.append(("r", "dx", rd, f"x1@{l}"))
             p.append(("w", "dx", rd, f"x2@{l}"))
             p.append(("barrier",))
