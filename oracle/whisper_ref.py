@@ -4,6 +4,9 @@ hot path, each citing the reference-side code it follows (TF = transformers 5.5.
   logmel_np              TF/models/whisper/feature_extraction_whisper.py:135-164 + TF/audio_utils.py (slaney bank)
   process_logits         TF/generation/logits_process.py:1812-1862 (begin suppress), :1865-1902 (suppress),
                          :1995-2043 (WhisperTimeStampLogitsProcessor)
+  select_greedy / beam_candidates
+                         the masks of process_logits, the probability rule in float64, greedy argmax + pad / finished
+                         (TF/generation/utils.py:2762-2797), one beam's top 2G (TF/generation/utils.py:3256-3257)
   median_filter / dtw / token_timestamps
                          TF/models/whisper/generation_whisper.py:43-61, :64-115, :331-379
 
@@ -77,6 +80,74 @@ def process_logits(scores: np.ndarray, seq: Sequence[int], begin_index: int, *, 
     if ts_lp > logp[:ts_begin].max():
         s[:ts_begin] = -np.inf
     return (s, pre, rule_margin) if details else s
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# token selection of one decoder step (decode.cu select_kernel, decode_mega.cu's fused greedy select), on exact logits
+# ------------------------------------------------------------------------------------------------------------------
+def rule_masks(V: int, seq: Sequence[int], begin_index: int, opts) -> np.ndarray:
+    """The ids process_logits masks before its probability rule, for history `seq` (bool [V]).  `opts` carries the fields
+    of thewhisper_b200.engine.DecodeOptions; max_initial_timestamp_index < 0 means no limit."""
+    mit = opts.max_initial_timestamp_index
+    _, pre, _ = process_logits(np.zeros(V, dtype=np.float32), seq, begin_index, suppress=list(opts.suppress_tokens),
+                               begin_suppress=list(opts.begin_suppress_tokens), ts_rules=bool(opts.timestamp_rules),
+                               ts_begin=opts.timestamp_begin, no_ts=opts.no_timestamps_token, eos=opts.eos_token,
+                               max_initial_ts=None if mit < 0 else mit, details=True)
+    return np.isneginf(pre)
+
+
+def _logsumexp(x: np.ndarray) -> float:
+    m = x.max() if len(x) else -np.inf
+    return float(m + np.log(np.exp(x - m).sum())) if np.isfinite(m) else -np.inf
+
+
+def _processed(vals: np.ndarray, seq, begin_index, opts, mask, rule_shift):
+    """float64 row with the masks applied and, under timestamp rules, the probability rule evaluated in float64:
+    logsumexp(timestamps) > max(text) masks all text.  -> (row, rule margin or nan).  rule_shift is added to the
+    timestamp side (tests use it to restate a wrong rule; -inf turns the rule off)."""
+    if mask is None:
+        mask = rule_masks(len(vals), seq, begin_index, opts)
+    s = np.where(mask, -np.inf, vals)
+    margin = float("nan")
+    if opts.timestamp_rules:
+        tb = opts.timestamp_begin
+        margin = _logsumexp(s[tb:]) - float(s[:tb].max())
+        if margin + rule_shift > 0:
+            s[:tb] = -np.inf
+    return s, margin
+
+
+def _order(s: np.ndarray, larger_id_ties: bool) -> np.ndarray:
+    ids = np.arange(len(s))
+    return np.lexsort((-ids if larger_id_ties else ids, -s))  # value descending, ties by id
+
+
+def select_greedy(row, seq, begin_index: int, finished: bool, opts, *, mask=None, rule_shift: float = 0.0,
+                  larger_id_ties: bool = False):
+    """Greedy step on one exact logit row -> (token, finished after the step, rule margin): the masks of process_logits,
+    the probability rule in float64, the first maximum (ties to the smaller id), then a finished row takes pad and a row
+    that chose eos becomes finished."""
+    s, margin = _processed(np.asarray(row, dtype=np.float64), seq, begin_index, opts, mask, rule_shift)
+    tok = int(_order(s, larger_id_ties)[0])
+    if finished:
+        return opts.pad_token, True, margin
+    return tok, tok == opts.eos_token, margin
+
+
+def beam_candidates(row, seq, begin_index: int, run: float, n: int, opts, *, mask=None, rule_shift: float = 0.0,
+                    larger_id_ties: bool = False):
+    """One sequence's best n continuations -> (scores float64 [n], ids [n], rule margin): log-softmax of the raw row in
+    float64 (HF takes it before the processors), the masks and probability rule on it (the rule is shift-invariant), plus
+    the running score `run`; ordered by (score descending, id ascending), missing entries (-inf, -1)."""
+    x = np.asarray(row, dtype=np.float64)
+    s, margin = _processed(x - _logsumexp(x), seq, begin_index, opts, mask, rule_shift)
+    s = s + run
+    top = _order(s, larger_id_ties)[:n]
+    top = top[np.isfinite(s[top])]
+    scores = np.full(n, -np.inf)
+    ids = np.full(n, -1, dtype=np.int64)
+    scores[:len(top)], ids[:len(top)] = s[top], top
+    return scores, ids, margin
 
 
 # ------------------------------------------------------------------------------------------------------------------
