@@ -93,6 +93,12 @@ int bw_engine_buffer(bw_engine* e, const char* name, void** device_ptr, size_t* 
 /* pcm: device fp32 [B, n_samples], n_samples == 320 * max_source_positions (chunk already zero-padded/truncated).
  * Writes the engine's mel buffer; if mel_f32_out != NULL also the reference layout [B, n_mels, frames] fp32. */
 int bw_logmel(bw_engine* e, const float* pcm, int32_t B, int32_t n_samples, float* mel_f32_out, void* stream);
+/* Features of audio of any length (sequential long-form transcription): pcm device fp32 [B, n_samples], every row zero-padded to the
+ * longest (n_samples >= 400).  Writes only mel_f32_out, device fp32 [B, n_mels, n_samples / 160] in the reference layout, with the
+ * "max - 8" clamp taken per row over the whole padded row (feature extractor with truncation=False, padding="longest"); the engine's
+ * mel buffer is not touched (windows of it go through bw_set_mel).  At n_samples = 320 * max_source_positions the values are
+ * bit-identical to bw_logmel's mel_f32_out. */
+int bw_logmel_long(bw_engine* e, const float* pcm, int32_t B, int32_t n_samples, float* mel_f32_out, void* stream);
 /* load externally computed features instead (device fp32 [B, n_mels, frames]) */
 int bw_set_mel(bw_engine* e, const float* mel_f32, int32_t B, void* stream);
 /* conv stem + encoder layers + final LayerNorm + cross-attention K/V projection of every decoder layer */
@@ -100,6 +106,13 @@ int bw_encode(bw_engine* e, int32_t B, void* stream);
 /* start a decode over A audios x G sequences; prompt_host: [A*G, prompt_len] int32 */
 int bw_decode_begin(bw_engine* e, int32_t A, int32_t G, const int32_t* prompt_host, int32_t prompt_len,
                     const bw_decode_opts* opts, void* stream);
+/* bw_decode_begin for left-padded decoder inputs: key_start_host [A] (or NULL = all 0), 0 <= key_start[a] < begin_index.  Positions
+ * below key_start[a] are absent as keys for every query of audio a's sequences, in every layer (transformers' decoder_attention_mask
+ * = ids != pad with the pads on the left; positions are not shifted).  Those keys are never read, so their K / V rows may hold
+ * anything; a query at such a position has no key and its attention output is 0.  A decode with a key start > 0 runs the per-op or
+ * batched step, never the persistent one; with every key start 0 it is exactly bw_decode_begin. */
+int bw_decode_begin_key_start(bw_engine* e, int32_t A, int32_t G, const int32_t* prompt_host, int32_t prompt_len,
+                              const bw_decode_opts* opts, const int32_t* key_start_host, void* stream);
 /* run n decoder steps (one CUDA-graph launch each, no host synchronisation).  Fails before launching anything when the
  * steps would run past position max_target_positions - 1 (counted from bw_decode_begin) */
 int bw_decode_run(bw_engine* e, int32_t n_steps, void* stream);
@@ -113,6 +126,10 @@ int bw_decode_prefill(bw_engine* e, int32_t n_positions, int32_t max_rows_per_pa
 /* kernels launched by bw_decode_run since the engine was created (kernel nodes of the step graph x graph launches);
  * bench.py reports it as part of "gpu_launches" */
 long long bw_decode_kernel_launches(bw_engine* e);
+/* step-graph cache since the engine was created: out[0] graphs captured, out[1] microseconds spent capturing and instantiating them
+ * (host clock), out[2] graphs cached now, out[3] graphs evicted.  The cache holds at most 64 graphs (BW_STEP_GRAPHS; 0 = unbounded)
+ * and evicts the least recently used one when a decode_begin needs a new graph. */
+int bw_decode_graph_stats(bw_engine* e, int64_t* out);
 /* synchronises the stream; tokens_host [A*G, max_target_positions], finished_host [A*G] (either may be NULL) */
 int bw_decode_read(bw_engine* e, int32_t* tokens_host, int32_t* finished_host, int32_t* pos_host, void* stream);
 /* beam search support: reorder sequences (new sequence i continues old sequence parent[i]) by permuting the

@@ -51,12 +51,15 @@ SYMBOLS = {
     "bw_engine_finalize": (C.c_int, [_P]),
     "bw_engine_buffer": (C.c_int, [_P, C.c_char_p, C.POINTER(_P), C.POINTER(C.c_size_t)]),
     "bw_logmel": (C.c_int, [_P, _P, _I, _I, _P, _P]),
+    "bw_logmel_long": (C.c_int, [_P, _P, _I, _I, _P, _P]),
     "bw_set_mel": (C.c_int, [_P, _P, _I, _P]),
     "bw_encode": (C.c_int, [_P, _I, _P]),
     "bw_decode_begin": (C.c_int, [_P, _I, _I, _P, _I, C.POINTER(bw_decode_opts), _P]),
+    "bw_decode_begin_key_start": (C.c_int, [_P, _I, _I, _P, _I, C.POINTER(bw_decode_opts), _P, _P]),
     "bw_decode_run": (C.c_int, [_P, _I, _P]),
     "bw_decode_prefill": (C.c_int, [_P, _I, _I, _P]),
     "bw_decode_kernel_launches": (C.c_longlong, [_P]),
+    "bw_decode_graph_stats": (C.c_int, [_P, C.POINTER(C.c_int64)]),
     "bw_decode_read": (C.c_int, [_P, _P, _P, _P, _P]),
     "bw_decode_reorder": (C.c_int, [_P, _P, _P, _P]),
     "bw_decode_beam_step": (C.c_int, [_P, _P, _P, _P, _P]),

@@ -24,7 +24,7 @@ def _topk_desc(values: np.ndarray, k: int) -> np.ndarray:
 
 
 def beam_search(eng, prompts: np.ndarray, A: int, G: int, opts, max_new: int, length_penalty: float = 1.0, return_beam_indices: bool = False,
-                prefill: bool = False):
+                prefill: bool = False, key_start=None):
     """prompts [A, plen] (prefill: teacher-forced positions in one batched prefill pass).  Returns (generated ids per audio (best beam, cut before EOS), n_steps, eos_seen) and, on request, the
     `beam_indices` of the returned sequences as GenerationMixin._beam_search keeps them (TF generation/utils.py:2984-2997,3065-3070):
     entry t = the global sequence slot (audio * G + beam) whose forward pass produced generated token t, -1 beyond the sequence."""
@@ -34,7 +34,10 @@ def beam_search(eng, prompts: np.ndarray, A: int, G: int, opts, max_new: int, le
     max_length = min(plen + max_new, Tmax)
     K = 2 * G
     rep = np.repeat(prompts, G, axis=0)
-    eng.decode_begin(rep, A, G, opts)
+    if key_start is None:
+        eng.decode_begin(rep, A, G, opts)
+    else:  # left-padded prompts: one key start per audio, shared by its beams
+        eng.decode_begin(rep, A, G, opts, key_start=key_start)
     if prefill and plen > 1:  # teacher-forced prompt positions
         eng.decode_prefill(plen - 1)
     else:

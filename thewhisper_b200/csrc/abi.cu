@@ -80,15 +80,23 @@ int bw_engine_buffer(bw_engine* e, const char* name, void** p, size_t* bytes) { 
 int bw_logmel(bw_engine* e, const float* pcm, int32_t B, int32_t n_samples, float* mel_f32_out, void* stream) {
   BW_FWD(bw_logmel, e, pcm, B, n_samples, mel_f32_out, stream);
 }
+int bw_logmel_long(bw_engine* e, const float* pcm, int32_t B, int32_t n_samples, float* mel_f32_out, void* stream) {
+  BW_FWD(bw_logmel_long, e, pcm, B, n_samples, mel_f32_out, stream);
+}
 int bw_set_mel(bw_engine* e, const float* mel, int32_t B, void* stream) { BW_FWD(bw_set_mel, e, mel, B, stream); }
 int bw_encode(bw_engine* e, int32_t B, void* stream) { BW_FWD(bw_encode, e, B, stream); }
 int bw_decode_begin(bw_engine* e, int32_t A, int32_t G, const int32_t* prompt, int32_t plen, const bw_decode_opts* opts, void* stream) {
   BW_FWD(bw_decode_begin, e, A, G, prompt, plen, opts, stream);
 }
+int bw_decode_begin_key_start(bw_engine* e, int32_t A, int32_t G, const int32_t* prompt, int32_t plen, const bw_decode_opts* opts,
+                              const int32_t* key_start, void* stream) {
+  BW_FWD(bw_decode_begin_key_start, e, A, G, prompt, plen, opts, key_start, stream);
+}
 int bw_decode_run(bw_engine* e, int32_t n_steps, void* stream) { BW_FWD(bw_decode_run, e, n_steps, stream); }
 int bw_decode_prefill(bw_engine* e, int32_t n_positions, int32_t max_rows_per_pass, void* stream) {
   BW_FWD(bw_decode_prefill, e, n_positions, max_rows_per_pass, stream);
 }
+int bw_decode_graph_stats(bw_engine* e, int64_t* out) { BW_FWD(bw_decode_graph_stats, e, out); }
 long long bw_decode_kernel_launches(bw_engine* e) {
   if (!e) return -1;
   return e->f16 ? bw_decode_kernel_launches_f16(BW_H(e)) : bw_decode_kernel_launches_bf16(BW_B(e));

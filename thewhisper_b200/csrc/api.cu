@@ -5,6 +5,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <chrono>
 #include <map>
 #include <string>
 #include <tuple>
@@ -60,11 +61,12 @@ struct DecLayer {
 
 // Everything a captured step graph bakes in as kernel parameters: a decode that differs in any of these gets its own graph
 // (round-1 advisor: eos / pad / timestamp ids were missing, a second decode with other ids replayed the old ones).
+// key_start: the decode has per-sequence key starts (a different path: no persistent step; the values themselves are device data)
 struct GraphKey {
-  int A, G, begin_index, ts_rules, align, variant, eos, pad, ts_begin, no_ts;
+  int A, G, begin_index, ts_rules, align, variant, eos, pad, ts_begin, no_ts, key_start;
   bool operator<(const GraphKey& o) const {
-    return std::tie(A, G, begin_index, ts_rules, align, variant, eos, pad, ts_begin, no_ts) <
-           std::tie(o.A, o.G, o.begin_index, o.ts_rules, o.align, o.variant, o.eos, o.pad, o.ts_begin, o.no_ts);
+    return std::tie(A, G, begin_index, ts_rules, align, variant, eos, pad, ts_begin, no_ts, key_start) <
+           std::tie(o.A, o.G, o.begin_index, o.ts_rules, o.align, o.variant, o.eos, o.pad, o.ts_begin, o.no_ts, o.key_start);
   }
 };
 
@@ -110,7 +112,17 @@ struct bw_engine {
   int steps = 0;  // decoder steps run since bw_decode_begin = the device's `pos` (a step at pos = Tmax would read and write row Tmax)
   bw_decode_opts opts{};
   bool use_anc = false;
+  // left-padded decoder inputs: key start of every sequence [Qm] on the device (keys below it are absent in every layer), valid when
+  // has_k0; has_k0 is false when every key start of the decode is 0, which then runs exactly the unmasked path
+  int* key_start = nullptr;
+  bool has_k0 = false;
   std::map<GraphKey, cudaGraphExec_t> graphs;
+  // step-graph cache, least recently used out first once it holds max_graphs (BW_STEP_GRAPHS, 0 = unbounded): conditioned long-form
+  // decoding makes a new begin_index (the longest row's history) almost every window, so an unbounded cache grows for as long as the
+  // process runs
+  std::map<GraphKey, long long> graph_used;  // key -> last decode_begin that used it
+  long long graph_tick = 0, graph_captures = 0, graph_capture_us = 0, graph_evictions = 0;
+  int max_graphs = 64;
   cudaGraphExec_t cur_graph = nullptr;
   std::map<cudaGraphExec_t, int> graph_kernels;  // kernel nodes of each captured step graph
   long long step_kernel_launches = 0;            // kernels launched by bw_decode_run so far (graph path)
@@ -306,6 +318,7 @@ int step_batched_impl(bw_engine* e, cudaStream_t st) {
       SelfAttnArgs s;
       s.qkv = e->dpart; s.nsplit = ns; s.split_stride = (long long)Q * 3 * D; s.qkv_bias = L.bqkv; s.q_alpha = 0.125f;
       s.kc = kc; s.vc = vc; s.kc_w = kc; s.vc_w = vc; s.anc = e->use_anc ? e->anc : nullptr; s.out_bf16 = e->dba; s.pos = e->pos;
+      s.k0 = e->has_k0 ? e->key_start : nullptr;
       s.H = H; s.D = D; s.Tmax = Tmax;
       if (int rc = launch_self_attn(st, s, Q)) return rc;
     }
@@ -372,7 +385,7 @@ int prefill_pass(bw_engine* e, cudaStream_t st, int t0, int n) {
                                          t0, Tmax))
       return rc;
     if (last) break;
-    if (int rc = launch_prefill_self_attn(st, e->pf_q, kc, vc, e->pf_a, Q, n, t0, H, Tmax)) return rc;
+    if (int rc = launch_prefill_self_attn(st, e->pf_q, kc, vc, e->pf_a, Q, n, t0, H, Tmax, e->has_k0 ? e->key_start : nullptr)) return rc;
     if (int rc = proj(e->pf_a, D, L.wo, L.sc[1], D, &ns)) return rc;
     if (int rc = launch_resid_ln(st, e->pf_x, e->pf_part, ns, (long long)R * D, L.bo, L.ln2g, L.ln2b, e->pf_n, R, D)) return rc;
     if (int rc = proj(e->pf_n, D, L.xwq, L.sc[2], D, &ns)) return rc;
@@ -410,7 +423,8 @@ int step_impl(bw_engine* e, cudaStream_t st) {
   const long long self_layer0 = (long long)e->cfg.max_audios * e->cfg.max_beams * Tmax * D;
   const long long cross_layer0 = (long long)e->cfg.max_audios * H * S * 64;
   bool mega_done = false, select_done = false;
-  if (!e->no_mega && G == 1 && Q <= 8 && (int)e->dec.size() <= MEGA_MAXL) {
+  // (key starts: the persistent step has no key mask; left padding only occurs at Q >= 2 with unequal histories)
+  if (!e->no_mega && !e->has_k0 && G == 1 && Q <= 8 && (int)e->dec.size() <= MEGA_MAXL) {
     // persistent one-kernel step (decode_mega.cu); falls through to the per-op path when unsupported (-3)
     MegaArgs m{};
     for (size_t l = 0; l < e->dec.size(); ++l) {
@@ -476,6 +490,7 @@ int step_impl(bw_engine* e, cudaStream_t st) {
     {
       SelfAttnArgs s;
       s.qkv = e->dqkv; s.kc = kc; s.vc = vc; s.anc = e->use_anc ? e->anc : nullptr; s.out = e->dattn; s.pos = e->pos;
+      s.k0 = e->has_k0 ? e->key_start : nullptr;
       s.H = H; s.D = D; s.Tmax = Tmax;
       if (int rc = launch_self_attn(st, s, Q)) return rc;
     }
@@ -640,6 +655,10 @@ int bw_engine_create(const bw_config* cfg, bw_engine** out) {
   e->no_mega = nm && nm[0] == '1';
   e->no_fused_select = getenv("BW_NO_FUSED_SELECT") != nullptr;
   {
+    const char* sg = getenv("BW_STEP_GRAPHS");
+    if (sg) e->max_graphs = atoi(sg);
+  }
+  {
     const char* fl = getenv("BW_MEGA_FLAGS");
     if (fl) e->mega_flags = atoi(fl);
   }
@@ -765,6 +784,7 @@ int bw_engine_finalize(bw_engine* e) {
   if (dalloc(e, "pos", &e->pos, 1)) return -1;
   if (dalloc(e, "anc", &e->anc, (size_t)Qm * Tmax)) return -1;
   if (dalloc(e, "anc_tmp", &e->anc_tmp, (size_t)Qm * Tmax)) return -1;
+  if (dalloc(e, "key_start", &e->key_start, (size_t)Qm)) return -1;
   if (dalloc(e, "done_ctr", &e->done_ctr, 1)) return -1;
   if (dalloc(e, "mega_bar", &e->mega_bar, 1024)) return -1;  // arrival counter [0] + per-CTA flags [32, 32 + SMs)
   {
@@ -833,6 +853,13 @@ int bw_logmel(bw_engine* e, const float* pcm, int32_t B, int32_t n_samples, floa
   return logmel(static_cast<cudaStream_t>(stream), e->mel_plan, pcm, B, n_samples, e->F, e->mel_tm, mel_f32_out, e->mel_scratch, e->mel_max);
 }
 
+int bw_logmel_long(bw_engine* e, const float* pcm, int32_t B, int32_t n_samples, float* mel_f32_out, void* stream) {
+  BW_CHECK(e && e->finalized && pcm && mel_f32_out, "bw_logmel_long: bad arguments");
+  BW_CHECK(B >= 1 && B <= e->cfg.max_audios, "bw_logmel_long: B=%d outside 1..%d", B, e->cfg.max_audios);
+  BW_CHECK(n_samples >= 400, "bw_logmel_long: n_samples=%d below one 400-sample frame", n_samples);
+  return logmel_long(static_cast<cudaStream_t>(stream), e->mel_plan, pcm, B, n_samples, mel_f32_out, e->mel_max);
+}
+
 int bw_set_mel(bw_engine* e, const float* mel, int32_t B, void* stream) {
   BW_CHECK(e && e->finalized && mel, "bw_set_mel: bad arguments");
   BW_CHECK(B >= 1 && B <= e->cfg.max_audios, "bw_set_mel: B=%d outside 1..%d", B, e->cfg.max_audios);
@@ -898,13 +925,30 @@ int bw_encode(bw_engine* e, int32_t B, void* stream) {
 }
 
 int bw_decode_begin(bw_engine* e, int32_t A, int32_t G, const int32_t* prompt, int32_t plen, const bw_decode_opts* opts, void* stream) {
+  return bw_decode_begin_key_start(e, A, G, prompt, plen, opts, nullptr, stream);
+}
+
+int bw_decode_begin_key_start(bw_engine* e, int32_t A, int32_t G, const int32_t* prompt, int32_t plen, const bw_decode_opts* opts,
+                              const int32_t* key_start, void* stream) {
   BW_CHECK(e && e->finalized && prompt && opts, "bw_decode_begin: bad arguments");
   BW_CHECK(A >= 1 && A <= e->cfg.max_audios && G >= 1 && G <= e->cfg.max_beams, "bw_decode_begin: A=%d G=%d out of range", A, G);
   BW_CHECK(plen >= 1 && plen <= e->Tmax, "bw_decode_begin: prompt_len=%d out of range", plen);
   BW_CHECK(opts->begin_index >= 1 && opts->begin_index <= plen, "bw_decode_begin: begin_index=%d outside 1..prompt_len", opts->begin_index);
+  bool has_k0 = false;
+  if (key_start)
+    for (int a = 0; a < A; ++a) {
+      BW_CHECK(key_start[a] >= 0 && key_start[a] < opts->begin_index, "bw_decode_begin: key_start[%d]=%d outside 0..begin_index-1 = 0..%d", a,
+               key_start[a], opts->begin_index - 1);
+      has_k0 |= key_start[a] > 0;
+    }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  e->A = A; e->G = G; e->Q = A * G; e->opts = *opts; e->use_anc = G > 1; e->steps = 0;
+  e->A = A; e->G = G; e->Q = A * G; e->opts = *opts; e->use_anc = G > 1; e->steps = 0; e->has_k0 = has_k0;
   const int Q = e->Q, Tmax = e->Tmax, V = e->V;
+  std::vector<int> k0v((size_t)Q, 0);
+  if (has_k0) {  // one key start per audio, shared by its G beams (a beam reorder stays within the audio: nothing to permute)
+    for (int q = 0; q < Q; ++q) k0v[q] = key_start[q / G];
+    BW_CUDA_OK(cudaMemcpyAsync(e->key_start, k0v.data(), sizeof(int) * Q, cudaMemcpyHostToDevice, st));
+  }
   std::vector<int> tok((size_t)Q * Tmax, opts->pad_token);
   for (int q = 0; q < Q; ++q) memcpy(&tok[(size_t)q * Tmax], prompt + (size_t)q * plen, sizeof(int) * plen);
   BW_CUDA_OK(cudaMemcpyAsync(e->tokens, tok.data(), tok.size() * sizeof(int), cudaMemcpyHostToDevice, st));
@@ -930,9 +974,22 @@ int bw_decode_begin(bw_engine* e, int32_t A, int32_t G, const int32_t* prompt, i
   if (!e->no_graph) {
     GraphKey key{A, G, opts->begin_index, opts->timestamp_rules * 4 + (opts->max_initial_timestamp_index + 1) * 8, opts->record_alignment,
                  e->mega_flags * 4 + (e->no_mega ? 1 : 0) + (e->no_fused_select ? 2 : 0),
-                 opts->eos_token, opts->pad_token, opts->timestamp_begin, opts->no_timestamps_token};
+                 opts->eos_token, opts->pad_token, opts->timestamp_begin, opts->no_timestamps_token, has_k0 ? 1 : 0};
     auto it = e->graphs.find(key);
     if (it == e->graphs.end()) {
+      // (the stream was synchronised above: no launch of an evicted graph is still in flight)
+      while (e->max_graphs > 0 && (int)e->graphs.size() >= e->max_graphs) {
+        auto lru = e->graph_used.begin();
+        for (auto u = e->graph_used.begin(); u != e->graph_used.end(); ++u)
+          if (u->second < lru->second) lru = u;
+        auto g = e->graphs.find(lru->first);
+        e->graph_kernels.erase(g->second);
+        cudaGraphExecDestroy(g->second);
+        e->graphs.erase(g);
+        e->graph_used.erase(lru);
+        ++e->graph_evictions;
+      }
+      const auto t_capture = std::chrono::steady_clock::now();
       cudaStream_t cs;
       BW_CUDA_OK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
       cudaGraph_t graph = nullptr;
@@ -973,7 +1030,11 @@ int bw_decode_begin(bw_engine* e, int32_t A, int32_t G, const int32_t* prompt, i
       e->graph_kernels[exec] = n_kernel_nodes;
       cudaStreamDestroy(cs);
       it = e->graphs.emplace(key, exec).first;
+      ++e->graph_captures;
+      e->graph_capture_us +=
+          std::chrono::duration_cast<std::chrono::microseconds>(std::chrono::steady_clock::now() - t_capture).count();
     }
+    e->graph_used[key] = ++e->graph_tick;
     e->cur_graph = it->second;
   }
   return 0;
@@ -1040,6 +1101,15 @@ int bw_decode_prefill(bw_engine* e, int32_t n_positions, int32_t max_rows_per_pa
 }
 
 long long bw_decode_kernel_launches(bw_engine* e) { return e ? e->step_kernel_launches : -1; }
+
+int bw_decode_graph_stats(bw_engine* e, int64_t* out) {
+  BW_CHECK(e && out, "bw_decode_graph_stats: bad arguments");
+  out[0] = e->graph_captures;
+  out[1] = e->graph_capture_us;
+  out[2] = (int64_t)e->graphs.size();
+  out[3] = e->graph_evictions;
+  return 0;
+}
 
 int bw_decode_read(bw_engine* e, int32_t* tokens_host, int32_t* finished_host, int32_t* pos_host, void* stream) {
   BW_CHECK(e && e->finalized && e->Q > 0, "bw_decode_read: no decode in progress");

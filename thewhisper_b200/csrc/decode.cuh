@@ -35,6 +35,9 @@ struct SelfAttnArgs {
   float* out = nullptr;        // [Q, D] fp32 (per-op GEMV path) ...
   bf16* out_bf16 = nullptr;    // ... or bf16 (operand of the batched path's wgmma out-projection); exactly one of the two
   const int* pos = nullptr;
+  // per-sequence key start [Q] (left-padded decoder inputs): keys at positions < k0[q] are absent for every query of sequence q and
+  // are never read; a query with no key (pos < k0[q]) writes zeros.  null = every key start is 0
+  const int* k0 = nullptr;
   int H = 0, D = 0, Tmax = 0;
   // batched path: the fused QKV GEMM leaves k / v of the current token in qkv (fp32, + bias); the (sequence, head) CTA rounds them to
   // bf16, appends them to the cache at position *pos and attends over them (the GEMV path appends in its own epilogue)
@@ -170,8 +173,10 @@ int launch_prefill_embed(cudaStream_t st, const void* E, const float* Es, const 
 // to the cache kc / vc [Q][Tmax][D]
 int launch_prefill_proj_sum(cudaStream_t st, const float* part, int nsplit, long long split_stride, const float* bias, int N, int D, int R,
                             bf16* qout, bf16* kc, bf16* vc, int n, int t0, int Tmax);
-// causal self-attention of the pass's rows over cache rows [0, t0 + i] of their sequence -> out [R][D]
-int launch_prefill_self_attn(cudaStream_t st, const bf16* q, const bf16* kc, const bf16* vc, bf16* out, int Q, int n, int t0, int H, int Tmax);
+// causal self-attention of the pass's rows over cache rows [k0[q], t0 + i] of their sequence -> out [R][D] (k0: per-sequence key start
+// [Q] on the device, or null = 0; a row with no key, t0 + i < k0[q], writes zeros)
+int launch_prefill_self_attn(cudaStream_t st, const bf16* q, const bf16* kc, const bf16* vc, bf16* out, int Q, int n, int t0, int H, int Tmax,
+                             const int* k0 = nullptr);
 // cross-attention: the G * n rows of audio a over its S encoder positions (kc / vc [A][H][S][64]) -> out [R][D]
 int launch_prefill_cross_attn(cudaStream_t st, const bf16* q, const bf16* kc, const bf16* vc, bf16* out, int A, int G, int n, int S, int H);
 

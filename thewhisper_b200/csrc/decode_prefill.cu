@@ -79,11 +79,14 @@ struct PfAttnParams {
   int H, D;
   float scale_log2e;
   bf16* out;      // [R][D]
+  const int* k0;  // causal: key start per sequence [Q] or null (keys below it are absent and never loaded)
 };
 
 // One CTA = 64 query rows of one (group, head).  Group z is sequence z (CAUSAL: keys = cache rows [0, t] of that sequence, a 3-D map
 // [Q][t0 + n][D] so that rows past the pass read as zeros) or audio z (keys = its S encoder positions, a 3-D map [A * H][S][64]).
 // Query tiles may run past their group into the next group's rows (or the map's zero fill): those rows are computed and not stored.
+// With a key start k0 (causal), key tiles start at row k0 of the sequence: the rows below it are never loaded, so whatever they hold
+// (left padding) cannot reach a valid row; a row with no visible key (t0 + i < k0) writes zeros.
 template <bool CAUSAL>
 __global__ void __launch_bounds__(PF_THREADS, 1)
 prefill_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
@@ -102,8 +105,9 @@ prefill_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   const int i0 = blockIdx.x * TQ, h = blockIdx.y, z = blockIdx.z;
   // keys this tile needs: causal, up to the position of its last row in the group; cross, all S
   const int last = min(i0 + TQ, p.rows) - 1;
-  const int n_keys = CAUSAL ? p.t0 + last + 1 : p.S;
-  const int NT = (n_keys + TK - 1) / TK;
+  const int kstart = (CAUSAL && p.k0) ? p.k0[z] : 0;
+  const int n_keys = CAUSAL ? p.t0 + last + 1 - kstart : p.S;
+  const int NT = n_keys > 0 ? (n_keys + TK - 1) / TK : 0;
 
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
@@ -129,8 +133,8 @@ prefill_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         mbar_wait_wg(&kv_empty[s], ((j / KV_STAGES) & 1) ^ 1);
         mbar_arrive_expect_tx(&kv_full[s], 2 * TILE_BYTES);
         if (CAUSAL) {
-          tma_load_3d(sK + s * TILE_BYTES, &tmK, &kv_full[s], h * DH, j * TK, z);
-          tma_load_3d(sV + s * TILE_BYTES, &tmV, &kv_full[s], h * DH, j * TK, z);
+          tma_load_3d(sK + s * TILE_BYTES, &tmK, &kv_full[s], h * DH, kstart + j * TK, z);
+          tma_load_3d(sV + s * TILE_BYTES, &tmV, &kv_full[s], h * DH, kstart + j * TK, z);
         } else {
           tma_load_3d(sK + s * TILE_BYTES, &tmK, &kv_full[s], 0, j * TK, z * p.H + h);
           tma_load_3d(sV + s * TILE_BYTES, &tmV, &kv_full[s], 0, j * TK, z * p.H + h);
@@ -167,7 +171,7 @@ prefill_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     wg_commit();
     wg_wait<0>();
     wg_pin(sc);
-    const int key0 = j * TK;
+    const int key0 = kstart + j * TK;
     if (key0 + TK - 1 > min(lim[0], lim[1])) {
 #pragma unroll
       for (int jj = 0; jj < TK / 8; ++jj)
@@ -186,9 +190,12 @@ prefill_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       for (int jj = 0; jj < TK / 8; ++jj) t = fmaxf(t, fmaxf(sc[4 * jj + 2 * hh], sc[4 * jj + 2 * hh + 1]));
       t = fmaxf(t, __shfl_xor_sync(0xffffffffu, t, 1));
       t = fmaxf(t, __shfl_xor_sync(0xffffffffu, t, 2));
-      const float m_new = fmaxf(m[hh], t);  // finite: key 0 is visible to every row, so tile 0 sets it
-      alpha[hh] = ex2_approx((m[hh] - m_new) * p.scale_log2e);
-      mb[hh] = m_new * p.scale_log2e;
+      // finite once the row has seen a key: the first key is visible to every row at or past the key start; a row below it keeps
+      // m = -inf and takes a zero reference, so that its probabilities are exactly 0 and never NaN
+      const float m_new = fmaxf(m[hh], t);
+      const float m_ref = m_new == -INFINITY ? 0.f : m_new;
+      alpha[hh] = ex2_approx((m[hh] - m_ref) * p.scale_log2e);
+      mb[hh] = m_ref * p.scale_log2e;
       m[hh] = m_new;
     }
     uint32_t pa[TK / 16][4];
@@ -224,7 +231,7 @@ prefill_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     float t = l[hh];
     t += __shfl_xor_sync(0xffffffffu, t, 1);
     t += __shfl_xor_sync(0xffffffffu, t, 2);
-    const float inv = 1.0f / t;
+    const float inv = t > 0.f ? 1.0f / t : 0.f;  // (t = 0: a row below its key start)
     const int i = i0 + r + 8 * hh;
     if (i < p.rows) {
       bf16* op = p.out + ((long long)(z * p.rows + i) * p.D + h * DH);
@@ -264,7 +271,8 @@ int launch_prefill_proj_sum(cudaStream_t st, const float* part, int nsplit, long
   return 0;
 }
 
-int launch_prefill_self_attn(cudaStream_t st, const bf16* q, const bf16* kc, const bf16* vc, bf16* out, int Q, int n, int t0, int H, int Tmax) {
+int launch_prefill_self_attn(cudaStream_t st, const bf16* q, const bf16* kc, const bf16* vc, bf16* out, int Q, int n, int t0, int H, int Tmax,
+                             const int* k0) {
   const int D = H * DH;
   CUtensorMap tmQ, tmK, tmV;
   if (int rc = make_tmap_2d_bf16(&tmQ, q, (uint64_t)Q * n, (uint64_t)D, (uint64_t)D * 2, TQ, DH)) return rc;
@@ -272,7 +280,7 @@ int launch_prefill_self_attn(cudaStream_t st, const bf16* q, const bf16* kc, con
   if (int rc = make_tmap_3d_bf16(&tmK, kc, (uint64_t)Q, (uint64_t)(t0 + n), (uint64_t)D, (uint64_t)D * 2, (uint64_t)Tmax * D * 2, TK, DH)) return rc;
   if (int rc = make_tmap_3d_bf16(&tmV, vc, (uint64_t)Q, (uint64_t)(t0 + n), (uint64_t)D, (uint64_t)D * 2, (uint64_t)Tmax * D * 2, TK, DH)) return rc;
   PfAttnParams p;
-  p.rows = n; p.n = n; p.t0 = t0; p.S = 0; p.H = H; p.D = D; p.scale_log2e = LOG2E; p.out = out;  // q already carries the 1/8
+  p.rows = n; p.n = n; p.t0 = t0; p.S = 0; p.H = H; p.D = D; p.scale_log2e = LOG2E; p.out = out; p.k0 = k0;  // q already carries the 1/8
   return launch_pf_attn<true>(st, tmQ, tmK, tmV, p, Q);
 }
 
@@ -284,7 +292,7 @@ int launch_prefill_cross_attn(cudaStream_t st, const bf16* q, const bf16* kc, co
   if (int rc = make_tmap_3d_bf16(&tmK, kc, (uint64_t)A * H, (uint64_t)S, DH, DH * 2, (uint64_t)S * DH * 2, TK, DH)) return rc;
   if (int rc = make_tmap_3d_bf16(&tmV, vc, (uint64_t)A * H, (uint64_t)S, DH, DH * 2, (uint64_t)S * DH * 2, TK, DH)) return rc;
   PfAttnParams p;
-  p.rows = G * n; p.n = n; p.t0 = 0; p.S = S; p.H = H; p.D = D; p.scale_log2e = LOG2E; p.out = out;
+  p.rows = G * n; p.n = n; p.t0 = 0; p.S = S; p.H = H; p.D = D; p.scale_log2e = LOG2E; p.out = out; p.k0 = nullptr;
   return launch_pf_attn<false>(st, tmQ, tmK, tmV, p, A);
 }
 

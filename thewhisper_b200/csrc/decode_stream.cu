@@ -273,7 +273,7 @@ __device__ __forceinline__ float block_sum4(float v, float* red4) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// causal self-attention over cached positions 0..pos of one (sequence, head).  128 threads = 16 key groups x 8 lanes;
+// causal self-attention over cached positions k0..pos of one (sequence, head) (k0 = the sequence's key start, 0 without one).  128 threads = 16 key groups x 8 lanes;
 // a lane owns 8 of the 64 head dims, so one warp-load covers 4 whole 128-byte K (or V) rows.  Keys are walked in chunks of 128
 // with an online softmax: 33 KB of static smem whatever Tmax is (holding all Tmax = 448 positions takes 116 KB: ONE CTA per SM);
 // all loads of a chunk in flight together.
@@ -291,11 +291,12 @@ __global__ void __launch_bounds__(128) self_attn_kernel(const SelfAttnArgs a) {
   pdl_launch();
   const int pos = *a.pos;
   const int n = pos + 1;
+  const int k0 = a.k0 ? a.k0[q] : 0;  // keys [k0, pos]; chunks start at k0, so no key below it is ever loaded
   const int grp = threadIdx.x >> 3, sub = threadIdx.x & 7;
   // batched path: k / v of this step come from the projection's output (qkv), are rounded to bf16, appended to the cache at
   // position pos (a sequence's newest row lives in its own slot) and attended over; the GEMV path appended them itself
   uint4 kw = make_uint4(0u, 0u, 0u, 0u), vw = kw;
-  const bool appender = a.kc_w && grp == (pos & 15);
+  const bool appender = a.kc_w && grp == ((pos - k0) & 15);  // the group that meets key pos in the chunk loop below
   if (appender) {
     const long long kidx = (long long)q * 3 * a.D + a.D + h * 64 + sub * 8;
     float kf[8], vf[8];
@@ -313,7 +314,7 @@ __global__ void __launch_bounds__(128) self_attn_kernel(const SelfAttnArgs a) {
   float acc[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-  for (int c0 = 0; c0 < n; c0 += SCH) {
+  for (int c0 = k0; c0 < n; c0 += SCH) {
     const int nc = min(SCH, n - c0);
     __syncthreads();  // everybody is done with the previous chunk's rows and probabilities
     for (int s = grp; s < nc; s += 16) {
@@ -374,7 +375,7 @@ __global__ void __launch_bounds__(128) self_attn_kernel(const SelfAttnArgs a) {
     float o = 0.f;
 #pragma unroll
     for (int g = 0; g < 16; ++g) o += redo[g][threadIdx.x];
-    const float r = o / l_run;
+    const float r = l_run > 0.f ? o / l_run : 0.f;  // (l_run = 0 only for a query below its key start: no key)
     if (a.out_bf16) a.out_bf16[(long long)q * a.D + h * 64 + threadIdx.x] = f2e(r);
     else a.out[(long long)q * a.D + h * 64 + threadIdx.x] = r;
   }

@@ -94,5 +94,8 @@ void logmel_plan_destroy(LogmelPlan* p);
 // scratch: B*(n_mels*frames) floats + B uints.
 int logmel(cudaStream_t st, const LogmelPlan* plan, const float* pcm, int B, int n_samples, int frames, bf16* out_tm,
            float* out_f32, float* scratch, unsigned* scratch_max);
+// any sample count: pcm [B, n_samples] (rows zero-padded to the longest) -> out_f32 [B, n_mels, n_samples / 160] fp32 only (the
+// reference layout; log10 values are written there and finalized in place, no scratch).  scratch_max: B uints.
+int logmel_long(cudaStream_t st, const LogmelPlan* plan, const float* pcm, int B, int n_samples, float* out_f32, unsigned* scratch_max);
 
 }  // namespace bw

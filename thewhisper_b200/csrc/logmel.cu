@@ -108,7 +108,7 @@ __device__ __forceinline__ float ord2f(unsigned o) {
 
 __global__ void __launch_bounds__(WARPS * 32)
 logmel_frames_kernel(LogmelPlan plan, const float* __restrict__ pcm, int n_samples, int frames, float* __restrict__ scratch,
-                     unsigned* __restrict__ smax) {
+                     long long f_stride, long long m_stride, unsigned* __restrict__ smax) {
   __shared__ float2 s_tw[NFFT];
   __shared__ float s_win[NFFT];
   __shared__ float2 s_buf[WARPS][2][NFFT];
@@ -147,14 +147,17 @@ logmel_frames_kernel(LogmelPlan plan, const float* __restrict__ pcm, int n_sampl
     float* pw = reinterpret_cast<float*>(b1);
     for (int i = lane; i < NBINS; i += 32) pw[i] = b0[i].x * b0[i].x + b0[i].y * b0[i].y;
     __syncwarp();
-    float* orow = scratch + ((long long)b * frames + f) * plan.n_mels;
+    // log10 of (audio b, frame f, mel m) goes to scratch[b * frames * n_mels + f * f_stride + m * m_stride]: time-major rows
+    // (f_stride = n_mels, m_stride = 1) on the chunk path, the reference's [mel][frame] layout (f_stride = 1, m_stride = frames)
+    // on the long path, which then finalizes in place
+    float* orow = scratch + (long long)b * frames * plan.n_mels + f * f_stride;
     for (int mth = lane; mth < plan.n_mels; mth += 32) {
       const int s = plan.fstart[mth], n = plan.flen[mth];
       const float* w = plan.fw + mth * MAXW;
       float acc = 0.f;
       for (int i = 0; i < n; ++i) acc = fmaf(w[i], pw[s + i], acc);
       const float lv = log10f(fmaxf(acc, 1e-10f));
-      orow[mth] = lv;
+      orow[mth * m_stride] = lv;
       wmax = fmaxf(wmax, lv);
     }
   }
@@ -199,6 +202,15 @@ __global__ void logmel_finalize_kernel(const float* __restrict__ scratch, const 
       if (f0 + ff < frames) out_f32[((long long)b * n_mels + mth) * frames + f0 + ff] = tile[ff][mth];
     }
   }
+}
+
+// long path: x [B][n_mels][frames] fp32 in place -> (max(x, max_b - 8) + 4) / 4, the arithmetic of logmel_finalize_kernel
+__global__ void logmel_finalize_inplace_kernel(float* __restrict__ x, const unsigned* __restrict__ smax, long long per_audio) {
+  const int b = blockIdx.y;
+  const float floor_v = ord2f(smax[b]) - 8.0f;
+  float* xb = x + (long long)b * per_audio;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < per_audio; i += (long long)gridDim.x * blockDim.x)
+    xb[i] = (fmaxf(xb[i], floor_v) + 4.0f) / 4.0f;
 }
 
 }  // namespace
@@ -264,10 +276,26 @@ int logmel(cudaStream_t st, const LogmelPlan* plan, const float* pcm, int B, int
   BW_CHECK(frames * HOP <= n_samples, "logmel: frames=%d exceeds n_samples/160", frames);
   BW_CUDA_OK(cudaMemsetAsync(scratch_max, 0, sizeof(unsigned) * B, st));
   dim3 g1((frames + WARPS - 1) / WARPS, B);
-  logmel_frames_kernel<<<g1, WARPS * 32, 0, st>>>(*plan, pcm, n_samples, frames, scratch, scratch_max);
+  logmel_frames_kernel<<<g1, WARPS * 32, 0, st>>>(*plan, pcm, n_samples, frames, scratch, plan->n_mels, 1, scratch_max);
   BW_CUDA_OK(cudaGetLastError());
   dim3 g2((frames + 31) / 32, B);
   logmel_finalize_kernel<<<g2, 256, 0, st>>>(scratch, scratch_max, frames, plan->n_mels, out_tm, out_f32);
+  BW_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int logmel_long(cudaStream_t st, const LogmelPlan* plan, const float* pcm, int B, int n_samples, float* out_f32, unsigned* scratch_max) {
+  BW_CHECK(plan != nullptr && out_f32 != nullptr, "logmel_long: null plan or output");
+  BW_CHECK(n_samples >= NFFT, "logmel_long: n_samples=%d too short", n_samples);
+  const int frames = n_samples / HOP;
+  BW_CUDA_OK(cudaMemsetAsync(scratch_max, 0, sizeof(unsigned) * B, st));
+  dim3 g1((frames + WARPS - 1) / WARPS, B);
+  logmel_frames_kernel<<<g1, WARPS * 32, 0, st>>>(*plan, pcm, n_samples, frames, out_f32, 1, frames, scratch_max);
+  BW_CUDA_OK(cudaGetLastError());
+  const long long per_audio = (long long)plan->n_mels * frames;
+  const long long blocks = (per_audio + 255) / 256;
+  dim3 g2((unsigned)(blocks < 1024 ? blocks : 1024), B);
+  logmel_finalize_inplace_kernel<<<g2, 256, 0, st>>>(out_f32, scratch_max, per_audio);
   BW_CUDA_OK(cudaGetLastError());
   return 0;
 }

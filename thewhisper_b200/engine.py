@@ -234,8 +234,9 @@ class WhisperEngine:
         self._pcm_pin = torch.empty((max_audios, self.n_samples), dtype=torch.float32).pin_memory()
         self._tok_host = np.zeros((max_audios * max_beams, dims.max_target_positions), dtype=np.int32)
         self._keep = None
+        self._keep_pcm = None
         # work counters (bench / diagnostics): the timestamp `seek` loop may encode and decode a chunk more than once
-        self.stats = {"encode_calls": 0, "chunks_encoded": 0, "decode_steps": 0, "sequence_steps": 0}
+        self.stats = {"encode_calls": 0, "chunks_encoded": 0, "decode_steps": 0, "sequence_steps": 0, "prefill_passes": 0}
 
     # ------------------------------------------------------------------------------------------
     def close(self):
@@ -291,6 +292,25 @@ class WhisperEngine:
                                       C.c_void_p(out.data_ptr()) if out is not None else None, self._stream()))
         return out
 
+    def logmel_long(self, pcm: np.ndarray) -> torch.Tensor:
+        """Features of audio of any length: pcm host float32 [B, L], every row zero-padded to the longest, L >= 400 ->
+        device fp32 [B, n_mels, L // 160] (the feature extractor's truncation=False, padding="longest" layout, clamp per row).
+        The PCM staging and the feature buffer are allocated per call, sized to the group (184 MB of features per hour of audio at
+        128 mels); when either allocation fails this raises before anything is launched.  The engine's mel buffer is untouched."""
+        pcm = np.ascontiguousarray(pcm, dtype=np.float32)
+        B, L = pcm.shape
+        assert B <= self.max_audios, (B, self.max_audios)
+        try:
+            pcm_dev = torch.empty((B, L), dtype=torch.float32, device=self.device)
+            out = torch.empty((B, self.dims.n_mels, L // HOP), dtype=torch.float32, device=self.device)
+        except torch.cuda.OutOfMemoryError as err:
+            raise _lib.BwError(f"logmel_long: cannot allocate the features of {B} x {L} samples "
+                               f"({(B * L + B * self.dims.n_mels * (L // HOP)) * 4 / 2**20:.0f} MiB): {err}") from None
+        pcm_dev.copy_(torch.from_numpy(pcm))
+        _lib.check(self.lib.bw_logmel_long(self.h, C.c_void_p(pcm_dev.data_ptr()), B, L, C.c_void_p(out.data_ptr()), self._stream()))
+        self._keep_pcm = pcm_dev  # the copy and the kernels are stream-ordered; the staging lives until the next call
+        return out
+
     def set_mel(self, mel: torch.Tensor) -> None:
         """Load externally computed features [B, n_mels, frames] (device fp32) instead of running bw_logmel."""
         mel = mel.to(device=self.device, dtype=torch.float32).contiguous()
@@ -307,7 +327,9 @@ class WhisperEngine:
         return self.buffer("enc_out", self.dtype, (self.max_audios, self.S, self.dims.d_model))[:B].float()
 
     # ------------------------------------------------------------------------------------------
-    def decode_begin(self, prompts: np.ndarray, A: int, G: int, opts: DecodeOptions, begin_index: Optional[int] = None) -> None:
+    def decode_begin(self, prompts: np.ndarray, A: int, G: int, opts: DecodeOptions, begin_index: Optional[int] = None,
+                     key_start: Optional[Sequence[int]] = None) -> None:
+        """key_start [A] (left-padded prompts): positions below key_start[a] are absent as keys for audio a's sequences."""
         prompts = np.ascontiguousarray(prompts, dtype=np.int32)
         assert prompts.shape[0] == A * G, (prompts.shape, A, G)
         plen = prompts.shape[1]
@@ -324,7 +346,13 @@ class WhisperEngine:
         o.begin_suppress_tokens = bsup.ctypes.data_as(C.POINTER(C.c_int32))
         o.n_begin_suppress = len(bsup)
         o.record_alignment = int(opts.record_alignment)
-        _lib.check(self.lib.bw_decode_begin(self.h, A, G, prompts.ctypes.data_as(C.c_void_p), plen, C.byref(o), self._stream()))
+        if key_start is None:
+            _lib.check(self.lib.bw_decode_begin(self.h, A, G, prompts.ctypes.data_as(C.c_void_p), plen, C.byref(o), self._stream()))
+        else:
+            ks = np.ascontiguousarray(key_start, dtype=np.int32)
+            assert ks.shape == (A,), (ks.shape, A)
+            _lib.check(self.lib.bw_decode_begin_key_start(self.h, A, G, prompts.ctypes.data_as(C.c_void_p), plen, C.byref(o),
+                                                          ks.ctypes.data_as(C.c_void_p), self._stream()))
         self._Q = A * G
         self._A = A
         self._plen = plen
@@ -339,6 +367,13 @@ class WhisperEngine:
         max_rows_per_pass = sequences x positions rows; 0 = the engine's default): the state n_positions decode_run steps
         leave, except the logits.  Must directly follow decode_begin; n_positions <= begin_index - 1."""
         _lib.check(self.lib.bw_decode_prefill(self.h, n_positions, max_rows_per_pass, self._stream()))
+        self.stats["prefill_passes"] += 1
+
+    def graph_stats(self) -> Dict[str, float]:
+        """The engine's step-graph cache: graphs captured, seconds spent capturing them, graphs cached now, graphs evicted."""
+        out = (C.c_int64 * 4)()
+        _lib.check(self.lib.bw_decode_graph_stats(self.h, out))
+        return {"captured": int(out[0]), "capture_s": out[1] / 1e6, "cached": int(out[2]), "evicted": int(out[3])}
 
     def decode_kernel_launches(self) -> int:
         """Kernels launched by decode_run so far (counted from the captured step graphs)."""
@@ -376,14 +411,14 @@ class WhisperEngine:
         return self.buffer("logits", torch.float32, (self.max_audios * self.max_beams, vp))[: self._Q, : self.dims.vocab]
 
     def greedy(self, prompts: np.ndarray, A: int, opts: DecodeOptions, max_new_tokens: int, poll_every: int = 32,
-               prefill: bool = False):
+               prefill: bool = False, key_start: Optional[Sequence[int]] = None):
         """Greedy decode of A audios (their cross K/V must be resident from encode()).  Returns generated ids per
         audio (prompt stripped, cut at and excluding EOS) and the raw token matrix.  prefill: run the teacher-forced
-        positions as one batched prefill pass instead of step by step."""
+        positions as one batched prefill pass instead of step by step.  key_start: see decode_begin."""
         plen = prompts.shape[1]
         Tmax = self.dims.max_target_positions
         max_new = max(0, min(max_new_tokens, Tmax - plen))
-        self.decode_begin(prompts, A, 1, opts)
+        self.decode_begin(prompts, A, 1, opts, key_start=key_start)
         if prefill and plen > 1:  # teacher-forced prompt positions 0..plen-2
             self.decode_prefill(plen - 1)
         else:

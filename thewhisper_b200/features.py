@@ -61,3 +61,10 @@ def num_valid_frames(n_audio_samples: int, n_samples: int) -> int:
     """Valid mel frames of a (possibly shorter) input = attention_mask[:, ::hop].sum() (feature_extraction :328-337)."""
     n = min(n_audio_samples, n_samples)
     return (n + HOP - 1) // HOP if n % HOP else n // HOP
+
+
+def long_form_frames(n_audio_samples: int, n_padded: int) -> int:
+    """Frames of one item in a long-form group zero-padded to n_padded samples = its row of the feature extractor's rescaled
+    attention mask summed (feature_extraction_whisper.py:328-337: attention_mask[:, ::hop], minus the last column when n_padded is
+    not a multiple of hop): the frames j < n_padded // hop with j * hop < n_audio_samples."""
+    return min((n_audio_samples + HOP - 1) // HOP, n_padded // HOP)

@@ -10,7 +10,13 @@ What is covered (everything the reference's ASRPipeline / LocalWhisperBackend re
     `seek` loop for unfinished segments (:785-903, :1976-2073)
   * return_token_timestamps: per-token times from the alignment heads (:241-381) with HF's row bookkeeping
   * beam search (num_beams > 1) via thewhisper_b200.beam, incl. token timestamps along the winner's ancestry (beam_indices)
-Not covered (SURVEY.md §8f3, long-form only): temperature fallback, condition_on_prev_tokens, no-speech skipping.
+  * sequential long-form transcription (features longer than one window): the same seek loop over each item's own frame count
+    (_retrieve_max_frames_and_seek), language detected once on the first window, batch reduction to the rows still active
+  * condition_on_prev_tokens: [<|startofprev|> or the prompt (prompt_condition_type="all-segments"), last 223 tokens of the
+    row's text] + init tokens, rows left-padded to the longest and the pads masked by a per-row key start in decoder
+    self-attention (:1853-1915); the conditioning positions run as one batched prefill pass
+Not covered (long-form only): temperature fallback, logprob / compression-ratio thresholds, no-speech skipping -- sampling is not
+part of the engine.
 """
 from __future__ import annotations
 
@@ -41,6 +47,7 @@ class GenerationSettings:
     is_multilingual: bool = True
     max_length: int = 448
     median_filter_width: int = 7
+    prev_sot_token_id: Optional[int] = None
 
     @staticmethod
     def from_hf(gc, config=None) -> "GenerationSettings":
@@ -56,7 +63,8 @@ class GenerationSettings:
             alignment_heads=[list(p) for p in (getattr(gc, "alignment_heads", None) or [])],
             max_initial_timestamp_index=mi, is_multilingual=bool(getattr(gc, "is_multilingual", True)),
             max_length=int(getattr(gc, "max_length", 448) or 448),
-            median_filter_width=int(getattr(config, "median_filter_width", 7)) if config is not None else 7)
+            median_filter_width=int(getattr(config, "median_filter_width", 7)) if config is not None else 7,
+            prev_sot_token_id=(int(gc.prev_sot_token_id) if getattr(gc, "prev_sot_token_id", None) is not None else None))
 
 
 def _language_token(language: str, st: GenerationSettings) -> int:
@@ -137,11 +145,15 @@ class WhisperGenerator:
         return np.asarray(rows, dtype=np.int32)
 
     # --------------------------------------------------------------------------------------------------------
-    def _decode(self, prompts: np.ndarray, A: int, opts: DecodeOptions, max_new: int, num_beams: int, prefill: bool = False):
+    def _decode(self, prompts: np.ndarray, A: int, opts: DecodeOptions, max_new: int, num_beams: int, prefill: bool = False,
+                key_start=None):
         """-> (list of generated id arrays cut before EOS, n_steps HF would have run, eos_seen per row).  prefill: the
-        teacher-forced positions run as one batched prefill pass (a prompt), not step by step."""
+        teacher-forced positions run as one batched prefill pass (a prompt), not step by step.  key_start [A]: left-padded
+        prompts, the positions below it are masked (engine.decode_begin)."""
         self._beam_indices = None
         kw = {"prefill": True} if prefill else {}
+        if key_start is not None:
+            kw["key_start"] = key_start
         if num_beams > 1:
             from .beam import beam_search
 
@@ -231,50 +243,10 @@ class WhisperGenerator:
         return segs, offset
 
     # --------------------------------------------------------------------------------------------------------
-    def generate(self, B: int, num_frames: Optional[np.ndarray] = None, mel_f32: Optional[torch.Tensor] = None,
-                 return_timestamps: bool = False, return_token_timestamps: bool = False, language=None, task=None,
-                 num_beams: int = 1, max_new_tokens: Optional[int] = None, extra_suppress: Sequence[int] = (),
-                 encoded: bool = False, prompt_ids=None, prompt_condition_type: Optional[str] = None):
-        """The engine's mel buffer must hold the B chunks (engine.logmel / set_mel).  Returns a dict with
-        "sequences" (list of int arrays: generated ids, prompt and EOS stripped), optionally "token_timestamps"
-        (list of float arrays aligned with sequences) and "segments".
-        prompt_ids (tensor, array or list of ids, e.g. from get_prompt_ids): decoded as prompt + init tokens on every window, as
-        transformers' short-form generate does (generation_whisper.py _prepare_decoder_input_ids); the prompt positions run through
-        the decoder in one batched prefill pass."""
-        eng, st = self.eng, self.st
-        if prompt_condition_type not in (None, "first-segment", "all-segments"):
-            raise ValueError(f"`prompt_condition_type={prompt_condition_type} does not exist. Make sure to set `prompt_condition_type` "
-                             "to one of first-segment, all-segments")
-        if prompt_condition_type == "all-segments":
-            raise NotImplementedError("prompt_condition_type='all-segments' needs condition_on_prev_tokens, which the engine does not implement")
-        prompt = None
-        if prompt_ids is not None:
-            if isinstance(prompt_ids, torch.Tensor):
-                prompt_ids = prompt_ids.detach().cpu().numpy()
-            prompt = np.asarray(prompt_ids, dtype=np.int64).reshape(-1).astype(np.int32)
-        F = eng.frames
-        if return_token_timestamps:
-            return_timestamps = True
-            if not eng.alignment_heads:
-                raise ValueError("Model generation config has no `alignment_heads`, token-level timestamps not available.")
-        if mel_f32 is None:
-            raise ValueError("generate needs the fp32 features (engine.logmel(..., return_f32=True)) for the seek loop")
-        if num_frames is None:
-            num_frames = np.full(B, F, dtype=np.int64)
-        num_frames = np.asarray(num_frames, dtype=np.int64)
-        if not encoded:
-            eng.encode(B)
-        prompts_all = self.init_tokens(B, language, task, return_timestamps)
-        if prompt is not None:  # decoder input = prompt + init tokens; begin_index, the length checks and timestamps count all of it
-            prompts_all = np.concatenate([np.repeat(prompt[None, :], B, axis=0), prompts_all], axis=1)
-        plen = prompts_all.shape[1]
-        mtp = eng.dims.max_target_positions
-        if max_new_tokens is not None:
-            max_new = max_new_tokens
-        elif prompt is not None:  # _set_max_new_tokens_and_length: max_length grows by the conditioning tokens, up to max_target_positions
-            max_new = min(st.max_length + min(mtp // 2 - 1, plen - 1), mtp) - plen
-        else:
-            max_new = st.max_length - plen
+    def _max_new(self, plen: int, n_init: int, max_new_tokens: Optional[int]) -> int:
+        """_set_max_new_tokens_and_length for a window whose decoder input is plen long (n_init of it init tokens): the length error,
+        then the default budget, which grows by the conditioning tokens (prompt / previous text) up to max_target_positions."""
+        st, mtp = self.st, self.eng.dims.max_target_positions
         if (max_new_tokens or 0) + plen > mtp:  # same check, same message as TF generation_whisper.py:1920-1930
             raise ValueError(
                 f"The length of `decoder_input_ids`, including special start tokens, prompt tokens, and previous tokens, is {plen}, "
@@ -283,19 +255,114 @@ class WhisperGenerator:
                 f"`max_target_positions` of the Whisper model: {mtp}. "
                 "You should either reduce the length of your prompt, or reduce the value of `max_new_tokens`, "
                 f"so that their combined length is less than {mtp}.")
-        if max_new + plen > mtp:  # (only the max_length default can get here)
-            max_new = mtp - plen
+        if max_new_tokens is not None:
+            max_new = max_new_tokens
+        elif plen > n_init:
+            max_new = min(st.max_length + min(mtp // 2 - 1, plen - 1), mtp) - plen
+        else:
+            max_new = st.max_length - plen
+        return min(max_new, mtp - plen)  # (only the max_length default can get past it)
+
+    def _previous_tokens(self, segs: list, bos: Optional[np.ndarray]) -> np.ndarray:
+        """One row of _pad_to_max_length(..., cut_off_length=max_target_positions // 2 - 1, skip_ending_double_timestamps=True)
+        before the padding: the row's segment tokens (a segment ending on two timestamps loses the last), the last 223 of them,
+        behind `bos` (<|startofprev|>, or the prompt with prompt_condition_type="all-segments")."""
+        tb, cut = self.timestamp_begin, self.eng.dims.max_target_positions // 2 - 1
+        parts = []
+        for d in segs:
+            t = np.asarray(d["tokens"], dtype=np.int64)
+            parts.append(t[:-1] if len(t) > 2 and t[-2] >= tb else t)
+        seq = np.concatenate(parts)[-cut:] if parts else np.zeros(0, dtype=np.int64)
+        if bos is not None:
+            seq = np.concatenate([bos.astype(np.int64), seq])
+        return seq
+
+    def generate(self, B: int, num_frames: Optional[np.ndarray] = None, mel_f32: Optional[torch.Tensor] = None,
+                 return_timestamps: bool = False, return_token_timestamps: bool = False, language=None, task=None,
+                 num_beams: int = 1, max_new_tokens: Optional[int] = None, extra_suppress: Sequence[int] = (),
+                 encoded: bool = False, prompt_ids=None, prompt_condition_type: Optional[str] = None,
+                 max_frames: Optional[np.ndarray] = None, condition_on_prev_tokens: bool = False):
+        """Returns a dict with "sequences" (list of int arrays: generated ids, prompt and EOS stripped), optionally
+        "token_timestamps" (list of float arrays aligned with sequences) and "segments".
+
+        Short form (mel_f32 [B, n_mels, frames] of one window): the engine's mel buffer must hold the B chunks (engine.logmel /
+        set_mel).  Long form (mel_f32 longer than the window, engine.logmel_long): transformers' sequential algorithm -- each
+        window at `seek` is cut from mel_f32, encoded, decoded with the timestamp rules and split into segments, and `seek` moves to
+        the end of the last complete segment; max_frames [B] are the items' own frame counts (attention mask), num_frames
+        (token timestamps) default to them.  Long form requires timestamps (transformers' ValueError otherwise).
+        prompt_ids (tensor, array or list of ids, e.g. from get_prompt_ids): decoded as prompt + init tokens on the first window
+        (prompt_condition_type "first-segment") or on every window ("all-segments", needs condition_on_prev_tokens), as
+        transformers' generate does (generation_whisper.py _prepare_decoder_input_ids).
+        condition_on_prev_tokens: from the second window on, the decoder input of every row is [<|startofprev|> (or the prompt),
+        last 223 tokens of its text so far] + init tokens, the rows left-padded to the longest; the pads are masked by a key start
+        per row.  The conditioning positions run through the decoder in one batched prefill pass."""
+        eng, st = self.eng, self.st
+        if prompt_condition_type not in (None, "first-segment", "all-segments"):
+            raise ValueError(f"`prompt_condition_type={prompt_condition_type} does not exist. Make sure to set `prompt_condition_type` "
+                             "to one of first-segment, all-segments")
+        if prompt_condition_type == "all-segments" and not condition_on_prev_tokens:
+            raise NotImplementedError("prompt_condition_type='all-segments' needs condition_on_prev_tokens=True")
+        all_segments = prompt_condition_type == "all-segments"
+        prompt = None
+        if prompt_ids is not None:
+            if isinstance(prompt_ids, torch.Tensor):
+                prompt_ids = prompt_ids.detach().cpu().numpy()
+            prompt = np.asarray(prompt_ids, dtype=np.int64).reshape(-1).astype(np.int32)
+        F = eng.frames
+        if mel_f32 is None:
+            raise ValueError("generate needs the fp32 features (engine.logmel(..., return_f32=True)) for the seek loop")
+        total_frames = int(mel_f32.shape[-1])
+        long_form = total_frames > F
+        if long_form:
+            if not return_timestamps:  # _set_return_timestamps, same message
+                raise ValueError(
+                    "You have passed more than 3000 mel input features (> 30 seconds) which automatically "
+                    "enables long-form generation which requires the model to predict timestamp tokens. Please "
+                    "either pass `return_timestamps=True` or make sure to pass no more than 3000 mel input features.")
+            return_timestamps = True
+        if return_token_timestamps:
+            return_timestamps = True
+            if not eng.alignment_heads:
+                raise ValueError("Model generation config has no `alignment_heads`, token-level timestamps not available.")
+        max_frames = np.full(B, total_frames, dtype=np.int64) if max_frames is None else np.asarray(max_frames, dtype=np.int64)
+        if num_frames is None:
+            num_frames = max_frames if long_form else np.full(B, F, dtype=np.int64)
+        num_frames = np.asarray(num_frames, dtype=np.int64)
+        # the encoder output of mel_f32[:, :, :F] for all B rows is resident: short form (the engine's mel buffer), or long form
+        # when the language is detected (once, on the first window, as transformers' detect_language reads it)
+        resident = encoded
+        if not long_form and not encoded:
+            eng.encode(B)
+            resident = True
+        detect = not isinstance(language, (list, tuple)) and language is None and bool(st.lang_to_id) and st.is_multilingual
+        if long_form and detect and not resident:
+            eng.set_mel(mel_f32[:, :, :F])
+            eng.encode(B)
+            resident = True
+        init_all = self.init_tokens(B, language, task, return_timestamps)
+        n_init = init_all.shape[1]
         opts = self._opts(return_timestamps, return_token_timestamps, extra_suppress)
+        if max_new_tokens is not None or prompt is not None:
+            self._max_new(n_init + (len(prompt) if prompt is not None else 0), n_init, max_new_tokens)  # refused before any decode
+        # _prepare_segments: with a first-segment prompt every row's history starts with the prompt (without <|startofprev|>)
+        prev_sot = st.prev_sot_token_id if st.prev_sot_token_id is not None else (
+            int(st.suppress_tokens[-2]) if len(st.suppress_tokens) >= 2 else None)
+        segments: List[list] = [[] for _ in range(B)]
+        n_hidden = 0
+        if prompt is not None and not all_segments:
+            p0 = prompt[1:] if st.prev_sot_token_id is not None and int(prompt[0]) == st.prev_sot_token_id else prompt
+            segments = [[{"tokens": p0.astype(np.int64)}] for _ in range(B)]
+            n_hidden = 1
+        tb = self.timestamp_begin
+        self.window_stats = {"windows": 0, "conditioned": 0, "left_padded": 0, "history_cut": 0}
 
         seek = np.zeros(B, dtype=np.int64)
-        max_frames = np.full(B, F, dtype=np.int64)
-        segments: List[list] = [[] for _ in range(B)]
         first = True
         while (seek < max_frames).any():
             rows = [i for i in range(B) if seek[i] < max_frames[i]]
             A = len(rows)
             seek_num_frames = np.minimum(max_frames - seek, F)
-            if not (first and A == B):
+            if not (first and A == B and resident and all(seek[i] == 0 and seek_num_frames[i] == F for i in rows)):
                 # cut the remaining features of every active row, zero-pad to the window (:1831-1850), re-encode
                 seg = torch.zeros((A, eng.dims.n_mels, F), dtype=torch.float32, device=mel_f32.device)
                 for j, i in enumerate(rows):
@@ -304,14 +371,45 @@ class WhisperGenerator:
                 eng.set_mel(seg)
                 eng.encode(A)
             first = False
-            prompts = prompts_all[rows]
-            gen, n_steps, _ = self._decode(prompts, A, opts, max_new, num_beams, **({"prefill": True} if prompt is not None else {}))
+            # decoder input (_prepare_decoder_input_ids): conditioning once row 0 has a history, else prompt + init, else init
+            key_start = None
+            if condition_on_prev_tokens and len(segments[0]) > 0:
+                bos = prompt if (prompt is not None and all_segments) else (
+                    np.asarray([prev_sot], dtype=np.int64) if prev_sot is not None else None)
+                prev = [self._previous_tokens(segments[i], bos) for i in rows]
+                width = max(len(p) for p in prev)
+                ids = np.full((A, width), st.pad_token_id, dtype=np.int64)
+                for j, p in enumerate(prev):
+                    ids[j, width - len(p):] = p
+                prompts = np.concatenate([ids, init_all[rows]], axis=1).astype(np.int32)
+                valid = prompts != st.pad_token_id  # decoder_attention_mask; the pads sit on the left
+                ks = valid.argmax(axis=1)
+                if not all(valid[j, ks[j]:].all() for j in range(A)):
+                    raise NotImplementedError("a conditioning token equals pad_token_id: the decoder mask would not be a key start")
+                key_start = ks.astype(np.int32) if (ks > 0).any() else None
+                self.window_stats["conditioned"] += 1
+                self.window_stats["left_padded"] += int(key_start is not None)
+                cut = eng.dims.max_target_positions // 2 - 1
+                self.window_stats["history_cut"] += sum(
+                    sum(len(d["tokens"]) - (1 if len(d["tokens"]) > 2 and d["tokens"][-2] >= tb else 0) for d in segments[i]) > cut
+                    for i in rows)
+            elif prompt is not None:
+                prompts = np.concatenate([np.repeat(prompt[None, :], A, axis=0), init_all[rows]], axis=1)
+            else:
+                prompts = init_all[rows]
+            plen = prompts.shape[1]
+            max_new = self._max_new(plen, n_init, max_new_tokens)
+            self.window_stats["windows"] += 1
+            kw = {"prefill": True} if plen > n_init else {}
+            if key_start is not None:
+                kw["key_start"] = key_start
+            gen, n_steps, _ = self._decode(prompts, A, opts, max_new, num_beams, **kw)
             tts = None
             if return_token_timestamps:
                 tts = self._token_timestamps(A, plen, n_steps, (num_frames - seek)[rows])
             for j, i in enumerate(rows):
                 seq = np.asarray(gen[j], dtype=np.int64)
-                time_offset = float(seek[i]) * self.time_precision / 2.0
+                time_offset = float(seek[i]) * self.time_precision / 2.0  # (float64, as transformers computes it off the MPS device)
                 if len(seq) == 0:  # (HF runs _retrieve_segment in every mode: timestamp ids are not masked without timestamps)
                     s = {"start": time_offset, "end": time_offset + int(seek_num_frames[i] * 0.01 / self.time_precision) * self.time_precision,
                          "tokens": seq, "idxs": (plen, plen + len(seq))}
@@ -323,6 +421,7 @@ class WhisperGenerator:
                 segs, off = self._split_segments(seq, time_offset, int(seek_num_frames[i]), plen, tts[j] if tts is not None else None)
                 segments[i] += segs
                 seek[i] += off
+        segments = [segs[n_hidden:] for segs in segments]
         out = {"sequences": [np.concatenate([s["tokens"] for s in segs]) if segs else np.zeros(0, dtype=np.int64) for segs in segments],
                "segments": segments}
         if return_token_timestamps:

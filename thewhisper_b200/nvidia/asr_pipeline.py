@@ -6,6 +6,10 @@ model_size=None, chunk_length_s=30, device="cuda", torch_dtype=None, batch_size=
 `pipe(audio | [audio...] | {"raw"|"array", "sampling_rate"} | path | bytes, chunk_length_s=..., stride_length_s=...,
 return_timestamps=None|True|"word", return_language=..., batch_size=..., generate_kwargs={...})`
 -> `{"text": str, "chunks": [{"text", "timestamp": (start, end)}]}`.
+Without chunk_length_s, an input longer than the window is transcribed with Whisper's sequential long-form algorithm (as
+transformers' pipeline does): inputs are grouped batch_size at a time, a group whose longest item fits the window takes the
+one-window path, any other group the long-form seek loop of WhisperGenerator.generate (timestamps on; generate_kwargs
+condition_on_prev_tokens / prompt_condition_type as in transformers).
 
 Everything numeric below the call -- log-mel, encoder, decoder, logits rules, token selection, DTW -- runs in the CUDA
 engine through the C-ABI.  What stays on the host is what the reference keeps on the host too: the window schedule of
@@ -23,7 +27,7 @@ import numpy as np
 import torch
 
 from ..engine import ModelDims, WhisperEngine, engine_dtype
-from ..features import SAMPLE_RATE, num_valid_frames, pad_or_trim
+from ..features import SAMPLE_RATE, long_form_frames, num_valid_frames, pad_or_trim
 from ..generation import GenerationSettings, WhisperGenerator
 from ..hostproc import AsrDecoder, chunk_windows, install_merge
 
@@ -154,11 +158,7 @@ class ASRPipeline:
                 raise ValueError("Chunk length must be superior to stride length")
             for start, end, stride, is_last in chunk_windows(audio.shape[0], chunk_len, sl, sr):
                 yield audio[start:end], stride
-        else:
-            if audio.shape[0] > n_samples:
-                raise NotImplementedError(
-                    "sequential long-form transcription (input longer than the window without chunk_length_s) is outside this "
-                    "engine's scope (SURVEY.md §8 f3); pass chunk_length_s as the reference's own callers do")
+        else:  # the whole input: one window, or sequential long-form transcription when it is longer
             yield audio, None
 
     # ------------------------------------------------------------------------------------------------------------
@@ -178,6 +178,14 @@ class ASRPipeline:
                              "Use `return_timestamps='word'` or `return_timestamps=True` respectively.")
         if generate_kwargs.get("do_sample"):
             raise NotImplementedError("sampling is not part of the engine (greedy / beam only)")
+        temperature = generate_kwargs.get("temperature")
+        if isinstance(temperature, (list, tuple)) or (temperature is not None and temperature > 0.0):
+            raise NotImplementedError(f"temperature={temperature!r}: temperature fallback samples, and sampling is not part of the engine "
+                                      "(greedy / beam only)")
+        for name in ("logprob_threshold", "compression_ratio_threshold", "no_speech_threshold"):
+            if generate_kwargs.get(name) is not None:
+                raise NotImplementedError(f"{name} is not implemented: the engine has no temperature fallback or no-speech skipping")
+        condition = bool(generate_kwargs.get("condition_on_prev_tokens") or False)
         num_beams = int(generate_kwargs.get("num_beams", 1) or 1)
         if num_beams > self.max_beams:
             raise ValueError(f"num_beams={num_beams} exceeds the engine's max_beams={self.max_beams}")
@@ -199,16 +207,30 @@ class ASRPipeline:
         for b0 in range(0, len(flat), batch_size):
             group = flat[b0:b0 + batch_size]
             B = len(group)
-            pcm = np.stack([pad_or_trim(g["audio"], n_samples) for g in group])
-            num_frames = np.asarray([num_valid_frames(len(g["audio"]), n_samples) for g in group], dtype=np.int64)
-            mel = self.engine.logmel(pcm, return_f32=True)
+            longest = max(len(g["audio"]) for g in group)
+            if longest <= n_samples:  # one window per item
+                pcm = np.stack([pad_or_trim(g["audio"], n_samples) for g in group])
+                num_frames = np.asarray([num_valid_frames(len(g["audio"]), n_samples) for g in group], dtype=np.int64)
+                mel = self.engine.logmel(pcm, return_f32=True)
+                long_kw = {}
+            else:  # sequential long form: features of the group zero-padded to its longest item, each item's own frame count
+                pcm = np.stack([pad_or_trim(g["audio"], longest) for g in group])
+                num_frames = np.asarray([long_form_frames(len(g["audio"]), longest) for g in group], dtype=np.int64)
+                mel = self.engine.logmel_long(pcm)
+                if mel.shape[-1] > self.engine.frames:
+                    long_kw = {"max_frames": num_frames}
+                else:  # under 160 samples past the window: still one window of features (transformers' short form), which
+                    # generate encodes from the engine's mel buffer -- bw_logmel_long does not write it
+                    self.engine.set_mel(mel)
+                    long_kw = {}
             tm["windows_s"] += _time.perf_counter() - t_ph
             t_ph = _time.perf_counter()
             out = self.generator.generate(
                 B, num_frames=num_frames, mel_f32=mel, return_timestamps=bool(return_timestamps),
                 return_token_timestamps=(return_timestamps == "word"), language=generate_kwargs.get("language"),
                 task=generate_kwargs.get("task"), num_beams=num_beams, max_new_tokens=generate_kwargs.get("max_new_tokens"),
-                prompt_ids=generate_kwargs.get("prompt_ids"), prompt_condition_type=generate_kwargs.get("prompt_condition_type"))
+                prompt_ids=generate_kwargs.get("prompt_ids"), prompt_condition_type=generate_kwargs.get("prompt_condition_type"),
+                condition_on_prev_tokens=condition, **long_kw)
             for j, g in enumerate(group):
                 o: Dict[str, Any] = {"tokens": np.asarray(out["sequences"][j], dtype=np.int64)[None, :]}
                 if return_timestamps == "word":
