@@ -128,8 +128,18 @@ int bw_decode_prefill(bw_engine* e, int32_t n_positions, int32_t max_rows_per_pa
 long long bw_decode_kernel_launches(bw_engine* e);
 /* step-graph cache since the engine was created: out[0] graphs captured, out[1] microseconds spent capturing and instantiating them
  * (host clock), out[2] graphs cached now, out[3] graphs evicted.  The cache holds at most 64 graphs (BW_STEP_GRAPHS; 0 = unbounded)
- * and evicts the least recently used one when a decode_begin needs a new graph. */
+ * and evicts the least recently used one when a decode needs a new graph (at its first bw_decode_run). */
 int bw_decode_graph_stats(bw_engine* e, int64_t* out);
+/* Scores of the decode begun by bw_decode_begin (no-speech skipping), allowed only before its first step or prefill and refused
+ * otherwise before anything is launched.  Every step from then on also writes, for each sequence q at the index cur_len of the token
+ * it selects: lp[q, cur_len], the log-softmax of the processed logits (suppression, begin suppression, the timestamp rules with
+ * their forcing) at that token (0 for a finished row), and lmass[q, cur_len] = logsumexp(logits the processors allow) -
+ * logsumexp(raw logits).  The step that consumes position nospeech_pos (-1 = none, else < begin_index, generating or not) writes
+ * nsp[q] = softmax(raw logits)[nospeech_token].  Token selection is unchanged; the persistent step's fused selection is not
+ * used while scores are on (the step runs token selection as a kernel of its own).  The position is not part of the step graph. */
+int bw_decode_scores_enable(bw_engine* e, int32_t nospeech_pos, int32_t nospeech_token, void* stream);
+/* synchronises the stream; lp_host / lmass_host [A*G, max_target_positions], nsp_host [A*G] fp32 (any may be NULL) */
+int bw_decode_read_scores(bw_engine* e, float* lp_host, float* lmass_host, float* nsp_host, void* stream);
 /* synchronises the stream; tokens_host [A*G, max_target_positions], finished_host [A*G] (either may be NULL) */
 int bw_decode_read(bw_engine* e, int32_t* tokens_host, int32_t* finished_host, int32_t* pos_host, void* stream);
 /* beam search support: reorder sequences (new sequence i continues old sequence parent[i]) by permuting the

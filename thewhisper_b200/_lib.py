@@ -61,6 +61,8 @@ SYMBOLS = {
     "bw_decode_kernel_launches": (C.c_longlong, [_P]),
     "bw_decode_graph_stats": (C.c_int, [_P, C.POINTER(C.c_int64)]),
     "bw_decode_read": (C.c_int, [_P, _P, _P, _P, _P]),
+    "bw_decode_scores_enable": (C.c_int, [_P, _I, _I, _P]),
+    "bw_decode_read_scores": (C.c_int, [_P, _P, _P, _P, _P]),
     "bw_decode_reorder": (C.c_int, [_P, _P, _P, _P]),
     "bw_decode_beam_step": (C.c_int, [_P, _P, _P, _P, _P]),
     "bw_word_timestamps": (C.c_int, [_P, _I, _I, _I, C.c_double, _P, _P]),

@@ -24,10 +24,13 @@ def _topk_desc(values: np.ndarray, k: int) -> np.ndarray:
 
 
 def beam_search(eng, prompts: np.ndarray, A: int, G: int, opts, max_new: int, length_penalty: float = 1.0, return_beam_indices: bool = False,
-                prefill: bool = False, key_start=None):
+                prefill: bool = False, key_start=None, nospeech=None):
     """prompts [A, plen] (prefill: teacher-forced positions in one batched prefill pass).  Returns (generated ids per audio (best beam, cut before EOS), n_steps, eos_seen) and, on request, the
     `beam_indices` of the returned sequences as GenerationMixin._beam_search keeps them (TF generation/utils.py:2984-2997,3065-3070):
-    entry t = the global sequence slot (audio * G + beam) whose forward pass produced generated token t, -1 beyond the sequence."""
+    entry t = the global sequence slot (audio * G + beam) whose forward pass produced generated token t, -1 beyond the sequence.
+    nospeech = (position, token): scores on (engine.decode_scores_enable); the result then also holds, last, the returned sequences'
+    raw log-probs per generated token [A, max_length - plen] (candidate score minus its parent's running score), which with the
+    engine's lmass at the slots of `beam_indices` give the processed log-probs."""
     plen = prompts.shape[1]
     V = eng.dims.vocab
     Tmax = eng.dims.max_target_positions
@@ -38,7 +41,10 @@ def beam_search(eng, prompts: np.ndarray, A: int, G: int, opts, max_new: int, le
         eng.decode_begin(rep, A, G, opts)
     else:  # left-padded prompts: one key start per audio, shared by its beams
         eng.decode_begin(rep, A, G, opts, key_start=key_start)
-    if prefill and plen > 1:  # teacher-forced prompt positions
+    if nospeech is not None:  # the prefill stops before the no-speech position (engine.teacher_force)
+        eng.decode_scores_enable(*nospeech)
+        eng.teacher_force(plen, prefill, nospeech[0])
+    elif prefill and plen > 1:  # teacher-forced prompt positions
         eng.decode_prefill(plen - 1)
     else:
         eng.decode_run(plen - 1)
@@ -56,6 +62,8 @@ def beam_search(eng, prompts: np.ndarray, A: int, G: int, opts, max_new: int, le
     finished = np.zeros((A, G), dtype=bool)
     running_bidx = np.full((A, G, Tmax), -1, dtype=np.int32)
     bidx = running_bidx.copy()
+    running_tlp = np.zeros((A, G, Tmax), dtype=np.float32)  # raw log-prob of each generated token (scores on)
+    tlp = running_tlp.copy()
     unsat = np.ones((A, 1), dtype=bool)
     top_mask = np.arange(K) < G
     ar = np.arange(A)[:, None]  # row gathers below: x[ar, idx] picks whole [Tmax] rows (np.take_along_axis would build an [A, K, Tmax] index grid)
@@ -78,6 +86,9 @@ def beam_search(eng, prompts: np.ndarray, A: int, G: int, opts, max_new: int, le
         top_seq[:, :, cur_len] = top_tok
         top_bidx = running_bidx[ar, top_beam]
         top_bidx[:, :, cur_len - plen] = top_beam + (np.arange(A) * G)[:, None]
+        if nospeech is not None:
+            top_tlp = running_tlp[ar, top_beam]
+            top_tlp[:, :, cur_len - plen] = top_scores - running_scores[ar, top_beam]
         hits = (top_tok == opts.eos_token) | (cur_len + 1 >= max_length)
         # running beams of the next iteration
         run_lp = top_scores + hits.astype(np.float32) * NEG
@@ -85,6 +96,8 @@ def beam_search(eng, prompts: np.ndarray, A: int, G: int, opts, max_new: int, le
         running_seq = top_seq[ar, nxt]
         running_scores = np.take_along_axis(run_lp, nxt, 1)
         running_bidx = top_bidx[ar, nxt]
+        if nospeech is not None:
+            running_tlp = top_tlp[ar, nxt]
         parents = np.take_along_axis(top_beam, nxt, 1)
         next_tok = np.take_along_axis(top_tok, nxt, 1)
         # finished beams
@@ -99,6 +112,8 @@ def beam_search(eng, prompts: np.ndarray, A: int, G: int, opts, max_new: int, le
         sel = _topk_desc(m_scores, G)
         sequences = m_seq[ar, sel]
         bidx = m_bidx[ar, sel]
+        if nospeech is not None:
+            tlp = np.concatenate([tlp, top_tlp], 1)[ar, sel]
         beam_scores = np.take_along_axis(m_scores, sel, 1)
         finished = np.take_along_axis(m_fin, sel, 1)
         cur_len += 1
@@ -117,6 +132,9 @@ def beam_search(eng, prompts: np.ndarray, A: int, G: int, opts, max_new: int, le
         cut = np.where(row == opts.eos_token)[0]
         eos_seen.append(len(cut) > 0)
         gen.append(row[: cut[0]] if len(cut) else row)
+    out = (gen, steps, eos_seen)
     if return_beam_indices:
-        return gen, steps, eos_seen, bidx[:, 0, :].astype(np.int64)
-    return gen, steps, eos_seen
+        out += (bidx[:, 0, :].astype(np.int64),)
+    if nospeech is not None:
+        out += (tlp[:, 0, :],)
+    return out

@@ -102,6 +102,10 @@ long long bw_decode_kernel_launches(bw_engine* e) {
   return e->f16 ? bw_decode_kernel_launches_f16(BW_H(e)) : bw_decode_kernel_launches_bf16(BW_B(e));
 }
 int bw_decode_read(bw_engine* e, int32_t* tokens, int32_t* finished, int32_t* pos, void* stream) { BW_FWD(bw_decode_read, e, tokens, finished, pos, stream); }
+int bw_decode_scores_enable(bw_engine* e, int32_t nospeech_pos, int32_t nospeech_token, void* stream) {
+  BW_FWD(bw_decode_scores_enable, e, nospeech_pos, nospeech_token, stream);
+}
+int bw_decode_read_scores(bw_engine* e, float* lp, float* lmass, float* nsp, void* stream) { BW_FWD(bw_decode_read_scores, e, lp, lmass, nsp, stream); }
 int bw_decode_reorder(bw_engine* e, const int32_t* parent, const int32_t* next_token, void* stream) {
   BW_FWD(bw_decode_reorder, e, parent, next_token, stream);
 }

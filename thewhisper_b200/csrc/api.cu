@@ -63,10 +63,10 @@ struct DecLayer {
 // (round-1 advisor: eos / pad / timestamp ids were missing, a second decode with other ids replayed the old ones).
 // key_start: the decode has per-sequence key starts (a different path: no persistent step; the values themselves are device data)
 struct GraphKey {
-  int A, G, begin_index, ts_rules, align, variant, eos, pad, ts_begin, no_ts, key_start;
+  int A, G, begin_index, ts_rules, align, variant, eos, pad, ts_begin, no_ts, key_start, scores;
   bool operator<(const GraphKey& o) const {
-    return std::tie(A, G, begin_index, ts_rules, align, variant, eos, pad, ts_begin, no_ts, key_start) <
-           std::tie(o.A, o.G, o.begin_index, o.ts_rules, o.align, o.variant, o.eos, o.pad, o.ts_begin, o.no_ts, o.key_start);
+    return std::tie(A, G, begin_index, ts_rules, align, variant, eos, pad, ts_begin, no_ts, key_start, scores) <
+           std::tie(o.A, o.G, o.begin_index, o.ts_rules, o.align, o.variant, o.eos, o.pad, o.ts_begin, o.no_ts, o.key_start, o.scores);
   }
 };
 
@@ -116,11 +116,18 @@ struct bw_engine {
   // has_k0; has_k0 is false when every key start of the decode is 0, which then runs exactly the unmasked path
   int* key_start = nullptr;
   bool has_k0 = false;
+  // scores of the decode (bw_decode_scores_enable): lp / lmass [Qm][Tmax], nsp [Qm], nsp_cfg = {position, token} on the device
+  bool scores = false;
+  float *sc_lp = nullptr, *sc_lmass = nullptr, *sc_nsp = nullptr;
+  int* nsp_cfg = nullptr;
+  // the step graph is looked up (or captured) by the first bw_decode_run of a decode, so that bw_decode_scores_enable can still
+  // change its key
+  bool graph_pending = false;
   std::map<GraphKey, cudaGraphExec_t> graphs;
   // step-graph cache, least recently used out first once it holds max_graphs (BW_STEP_GRAPHS, 0 = unbounded): conditioned long-form
   // decoding makes a new begin_index (the longest row's history) almost every window, so an unbounded cache grows for as long as the
   // process runs
-  std::map<GraphKey, long long> graph_used;  // key -> last decode_begin that used it
+  std::map<GraphKey, long long> graph_used;  // key -> last decode that used it
   long long graph_tick = 0, graph_captures = 0, graph_capture_us = 0, graph_evictions = 0;
   int max_graphs = 64;
   cudaGraphExec_t cur_graph = nullptr;
@@ -451,7 +458,7 @@ int step_impl(bw_engine* e, cudaStream_t st) {
       m.align = e->align; m.Ha = e->cfg.n_align_heads; m.Tcap = e->cfg.max_align_steps; m.step_base = e->opts.begin_index;
     }
     m.trace = e->mega_trace;
-    if (!e->opts.timestamp_rules && !e->no_fused_select) {
+    if (!e->opts.timestamp_rules && !e->no_fused_select && !e->scores) {
       m.fuse_select = 1;
       m.suppress_bits = e->sup_bits; m.begin_suppress_bits = e->bsup_bits; m.begin_index = e->opts.begin_index;
       m.eos = e->opts.eos_token; m.pad = e->opts.pad_token; m.finished = e->finished; m.tokens_rw = e->tokens; m.pos_rw = e->pos;
@@ -565,6 +572,7 @@ int step_impl(bw_engine* e, cudaStream_t st) {
   s.begin_index = e->opts.begin_index; s.eos = e->opts.eos_token; s.pad = e->opts.pad_token;
   s.ts_rules = e->opts.timestamp_rules; s.ts_begin = e->opts.timestamp_begin; s.no_ts = e->opts.no_timestamps_token;
   s.max_initial_ts = e->opts.max_initial_timestamp_index; s.out_lse = e->lse;
+  if (e->scores) { s.out_lp = e->sc_lp; s.out_lmass = e->sc_lmass; s.out_nsp = e->sc_nsp; s.nsp_cfg = e->nsp_cfg; }
   if (G > 1) { s.n_cand = 2 * G; s.run_scores = e->run_scores; s.cand_scores = e->cand_scores; s.cand_tokens = e->cand_tokens; }
   return launch_select(st, s);
 }
@@ -810,6 +818,9 @@ int bw_engine_finalize(bw_engine* e) {
     if (dalloc(e, "dpart", &e->dpart, (size_t)Qm * DPART_PER_ROW)) return -1;
   }
   if (dalloc(e, "lse", &e->lse, (size_t)Qm)) return -1;
+  if (dalloc(e, "sc_lp", &e->sc_lp, (size_t)Qm * e->Tmax) || dalloc(e, "sc_lmass", &e->sc_lmass, (size_t)Qm * e->Tmax) ||
+      dalloc(e, "sc_nsp", &e->sc_nsp, (size_t)Qm) || dalloc(e, "nsp_cfg", &e->nsp_cfg, 2))
+    return -1;
   if (dalloc(e, "run_scores", &e->run_scores, (size_t)Qm)) return -1;
   if (dalloc(e, "cand_scores", &e->cand_scores, (size_t)Qm * 16)) return -1;
   if (dalloc(e, "cand_tokens", &e->cand_tokens, (size_t)Qm * 16)) return -1;
@@ -971,13 +982,24 @@ int bw_decode_begin_key_start(bw_engine* e, int32_t A, int32_t G, const int32_t*
   BW_CUDA_OK(cudaGetLastError());
   BW_CUDA_OK(cudaStreamSynchronize(st));  // host staging vectors go out of scope
   e->cur_graph = nullptr;
-  if (!e->no_graph) {
+  e->scores = false;
+  e->graph_pending = !e->no_graph;
+  return 0;
+}
+
+// The step graph of the current decode, from the cache or captured now.  Called by the first bw_decode_run after bw_decode_begin:
+// every launch of an earlier decode's graph was synchronised by bw_decode_begin, and nothing since has launched one, so none of an
+// evicted graph is still in flight.
+static int acquire_step_graph(bw_engine* e) {
+  e->graph_pending = false;
+  const bw_decode_opts* opts = &e->opts;
+  const int A = e->A, G = e->G;
+  {
     GraphKey key{A, G, opts->begin_index, opts->timestamp_rules * 4 + (opts->max_initial_timestamp_index + 1) * 8, opts->record_alignment,
                  e->mega_flags * 4 + (e->no_mega ? 1 : 0) + (e->no_fused_select ? 2 : 0),
-                 opts->eos_token, opts->pad_token, opts->timestamp_begin, opts->no_timestamps_token, has_k0 ? 1 : 0};
+                 opts->eos_token, opts->pad_token, opts->timestamp_begin, opts->no_timestamps_token, e->has_k0 ? 1 : 0, e->scores ? 1 : 0};
     auto it = e->graphs.find(key);
     if (it == e->graphs.end()) {
-      // (the stream was synchronised above: no launch of an evicted graph is still in flight)
       while (e->max_graphs > 0 && (int)e->graphs.size() >= e->max_graphs) {
         auto lru = e->graph_used.begin();
         for (auto u = e->graph_used.begin(); u != e->graph_used.end(); ++u)
@@ -1045,6 +1067,8 @@ int bw_decode_run(bw_engine* e, int32_t n_steps, void* stream) {
   BW_CHECK(n_steps >= 0 && n_steps <= e->Tmax - e->steps, "bw_decode_run: %d steps from position %d would run past the last position %d",
            n_steps, e->steps, e->Tmax - 1);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (n_steps > 0 && e->graph_pending)
+    if (int rc = acquire_step_graph(e)) return rc;
   for (int i = 0; i < n_steps; ++i, ++e->steps) {
     if (e->cur_graph) {
       BW_CUDA_OK(cudaGraphLaunch(e->cur_graph, st));
@@ -1097,6 +1121,34 @@ int bw_decode_prefill(bw_engine* e, int32_t n_positions, int32_t max_rows_per_pa
   set_pos_kernel<<<1, 1, 0, st>>>(e->pos, n_positions);
   BW_CUDA_OK(cudaGetLastError());
   e->steps = n_positions;
+  return 0;
+}
+
+int bw_decode_scores_enable(bw_engine* e, int32_t nospeech_pos, int32_t nospeech_token, void* stream) {
+  BW_CHECK(e && e->finalized && e->Q > 0, "bw_decode_scores_enable: no decode in progress");
+  BW_CHECK(e->steps == 0, "bw_decode_scores_enable: a step or prefill has run since bw_decode_begin; scores must be enabled before it");
+  BW_CHECK(nospeech_pos >= -1 && nospeech_pos <= e->opts.begin_index - 1, "bw_decode_scores_enable: nospeech_pos=%d outside -1..begin_index-1 = -1..%d",
+           nospeech_pos, e->opts.begin_index - 1);
+  BW_CHECK(nospeech_token >= 0 && nospeech_token < e->V, "bw_decode_scores_enable: nospeech_token=%d outside 0..%d", nospeech_token, e->V - 1);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int cfg[2] = {nospeech_pos, nospeech_token};
+  BW_CUDA_OK(cudaMemcpyAsync(e->nsp_cfg, cfg, sizeof(cfg), cudaMemcpyHostToDevice, st));
+  BW_CUDA_OK(cudaMemsetAsync(e->sc_lp, 0, sizeof(float) * e->Q * e->Tmax, st));
+  BW_CUDA_OK(cudaMemsetAsync(e->sc_lmass, 0, sizeof(float) * e->Q * e->Tmax, st));
+  BW_CUDA_OK(cudaMemsetAsync(e->sc_nsp, 0, sizeof(float) * e->Q, st));
+  BW_CUDA_OK(cudaStreamSynchronize(st));  // cfg is a host local
+  e->scores = true;
+  return 0;
+}
+
+int bw_decode_read_scores(bw_engine* e, float* lp_host, float* lmass_host, float* nsp_host, void* stream) {
+  BW_CHECK(e && e->finalized && e->Q > 0 && e->scores, "bw_decode_read_scores: no decode with scores in progress");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t n = (size_t)e->Q * e->Tmax;
+  if (lp_host) BW_CUDA_OK(cudaMemcpyAsync(lp_host, e->sc_lp, sizeof(float) * n, cudaMemcpyDeviceToHost, st));
+  if (lmass_host) BW_CUDA_OK(cudaMemcpyAsync(lmass_host, e->sc_lmass, sizeof(float) * n, cudaMemcpyDeviceToHost, st));
+  if (nsp_host) BW_CUDA_OK(cudaMemcpyAsync(nsp_host, e->sc_nsp, sizeof(float) * e->Q, cudaMemcpyDeviceToHost, st));
+  BW_CUDA_OK(cudaStreamSynchronize(st));
   return 0;
 }
 

@@ -75,6 +75,33 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(const SelectArgs a)
   const int pos = *a.pos;          // index of the token just consumed
   const int cur_len = pos + 1;     // tokens present; the new token goes to index cur_len
   const bool generating = cur_len >= a.begin_index && cur_len < a.Tmax;
+  const bool want_nsp = a.out_lp && pos == a.nsp_cfg[0];
+  if (!generating && want_nsp) {
+    // a forced step whose input is <|startoftranscript|> (a prompt or history before it): only the raw lse, for the no-speech prob
+    const float* lg = a.logits + (long long)q * a.ldl;
+    float m = -INFINITY;
+    for (int v = threadIdx.x; v < a.V; v += SEL_THREADS) m = fmaxf(m, lg[v]);
+    m = warp_max(m);
+    if (lane == 0) s_sum[warp] = m;
+    __syncthreads();
+    if (warp == 0) {
+      const float r = warp_max(s_sum[lane]);
+      if (lane == 0) s_f[0] = r;
+    }
+    __syncthreads();
+    m = s_f[0];
+    __syncthreads();
+    float sum = 0.f;
+    for (int v = threadIdx.x; v < a.V; v += SEL_THREADS) sum += __expf(lg[v] - m);
+    sum = warp_sum(sum);
+    if (lane == 0) s_sum[warp] = sum;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float rsum = 0.f;
+      for (int w = 0; w < SEL_THREADS / 32; ++w) rsum += s_sum[w];
+      a.out_nsp[q] = expf(lg[a.nsp_cfg[1]] - (m + logf(rsum)));
+    }
+  }
   if (generating) {
     const float* lg = a.logits + (long long)q * a.ldl;
     const int* seq = a.tokens + q * a.Tmax;
@@ -147,15 +174,19 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(const SelectArgs a)
     rawmax = s_f[0];
     __syncthreads();
     // ---- pass 2: sum exp over unmasked timestamps (relative to their max) and over all raw logits
-    float ts_sum = 0.f, raw_sum = 0.f;
+    //      (+ with scores on: over unmasked text, relative to its max -- the allowed mass)
+    const bool scores = a.out_lp != nullptr;
+    float ts_sum = 0.f, raw_sum = 0.f, text_sum = 0.f;
     for (int v = threadIdx.x; v < a.V; v += SEL_THREADS) {
       const float x = lg[v];
       raw_sum += __expf(x - rawmax);
       if (v >= tsb && !masked(v)) ts_sum += __expf(x - bs.v);
+      if (scores && v < tsb && !masked(v)) text_sum += __expf(x - bt.v);
     }
     ts_sum = warp_sum(ts_sum);
     raw_sum = warp_sum(raw_sum);
-    if (lane == 0) { s_sum[warp] = ts_sum; s_text[warp].v = raw_sum; }
+    if (scores) text_sum = warp_sum(text_sum);
+    if (lane == 0) { s_sum[warp] = ts_sum; s_text[warp].v = raw_sum; s_ts[warp].v = text_sum; }
     __syncthreads();
     if (threadIdx.x == 0) {
       float tsum = 0.f, rsum = 0.f;
@@ -172,7 +203,25 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(const SelectArgs a)
       } else {
         choice = bt.i;
       }
-      if (a.finished[q]) choice = a.pad;
+      const bool was_finished = a.finished[q] != 0;
+      if (scores) {
+        // log-softmax of the processed scores: the allowed set is the unmasked timestamps alone when a timestamp is forced
+        float xsum = 0.f;
+        for (int w = 0; w < SEL_THREADS / 32; ++w) xsum += s_ts[w].v;
+        const float raw_lse = rawmax + logf(rsum);
+        const float ts_lse = (bs.v == -INFINITY) ? -INFINITY : bs.v + logf(tsum);
+        const float text_lse = (bt.v == -INFINITY) ? -INFINITY : bt.v + logf(xsum);
+        const bool forced = a.ts_rules && ts_lse > bt.v;
+        float allowed = ts_lse;
+        if (!forced && text_lse != -INFINITY) {
+          const float hi = fmaxf(text_lse, ts_lse), lo = fminf(text_lse, ts_lse);
+          allowed = (lo == -INFINITY) ? hi : hi + log1pf(expf(lo - hi));
+        }
+        a.out_lmass[q * a.Tmax + cur_len] = allowed - raw_lse;
+        a.out_lp[q * a.Tmax + cur_len] = was_finished ? 0.f : (choice < a.V ? lg[choice] - allowed : -INFINITY);  // (none allowed)
+        if (want_nsp) a.out_nsp[q] = expf(lg[a.nsp_cfg[1]] - raw_lse);
+      }
+      if (was_finished) choice = a.pad;
       else if (choice == a.eos) a.finished[q] = 1;
       a.tokens[q * a.Tmax + cur_len] = choice;
       s_f[1] = rawmax + logf(rsum);

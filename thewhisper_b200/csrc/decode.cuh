@@ -90,6 +90,13 @@ struct SelectArgs {
   int eos = 0, pad = 0;
   int ts_rules = 0, ts_begin = 0, no_ts = 0, max_initial_ts = -1;
   float* out_lse = nullptr;  // optional [Q]: log-sum-exp of the raw logits (parity / beam search)
+  // optional scores (no-speech skipping), all set or all null: out_lp [Q, Tmax] the processed log-prob of the selected token (0 for a
+  // finished row), out_lmass [Q, Tmax] logsumexp(logits the processors allow) - logsumexp(raw logits), both at index cur_len;
+  // out_nsp [Q] softmax(raw)[nsp_cfg[1]] at the step that consumes position nsp_cfg[0] (device ints, so a graph serves any position)
+  float* out_lp = nullptr;
+  float* out_lmass = nullptr;
+  float* out_nsp = nullptr;
+  const int* nsp_cfg = nullptr;
   // beam search: per sequence the n_cand (<= 16) best continuations, running score included
   int n_cand = 0;
   const float* run_scores = nullptr;  // [Q]

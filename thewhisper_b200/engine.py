@@ -236,7 +236,10 @@ class WhisperEngine:
         self._keep = None
         self._keep_pcm = None
         # work counters (bench / diagnostics): the timestamp `seek` loop may encode and decode a chunk more than once
-        self.stats = {"encode_calls": 0, "chunks_encoded": 0, "decode_steps": 0, "sequence_steps": 0, "prefill_passes": 0}
+        # sot_split_steps: teacher-forced positions run as decoder steps instead of in the prefill, so that the no-speech probability
+        # can be read at the <|startoftranscript|> position (teacher_force)
+        self.stats = {"encode_calls": 0, "chunks_encoded": 0, "decode_steps": 0, "sequence_steps": 0, "prefill_passes": 0,
+                      "sot_split_steps": 0}
 
     # ------------------------------------------------------------------------------------------
     def close(self):
@@ -369,6 +372,36 @@ class WhisperEngine:
         _lib.check(self.lib.bw_decode_prefill(self.h, n_positions, max_rows_per_pass, self._stream()))
         self.stats["prefill_passes"] += 1
 
+    def decode_scores_enable(self, nospeech_pos: int = -1, nospeech_token: int = 0) -> None:
+        """Scores for the decode just begun (before its first step or prefill): every step also records the processed log-prob of
+        the token it selects and the allowed mass (see decode_scores); the step that consumes position nospeech_pos (-1 = none)
+        records softmax(raw logits)[nospeech_token].  Token selection is unchanged."""
+        _lib.check(self.lib.bw_decode_scores_enable(self.h, int(nospeech_pos), int(nospeech_token), self._stream()))
+
+    def decode_scores(self):
+        """-> (lp [Q, Tmax], lmass [Q, Tmax], nsp [Q]) float32 of the decode with scores on: lp[q, t] the log-softmax of the processed
+        logits at the token selected at index t (0 for a finished row), lmass[q, t] = logsumexp(allowed logits) - logsumexp(raw logits)
+        of that step (so a candidate's processed log-prob is its raw log-prob minus lmass), nsp[q] the no-speech probability."""
+        Q, T = self._Q, self.dims.max_target_positions
+        lp = np.empty((Q, T), dtype=np.float32)
+        lmass = np.empty((Q, T), dtype=np.float32)
+        nsp = np.empty(Q, dtype=np.float32)
+        _lib.check(self.lib.bw_decode_read_scores(self.h, lp.ctypes.data_as(C.c_void_p), lmass.ctypes.data_as(C.c_void_p),
+                                                  nsp.ctypes.data_as(C.c_void_p), self._stream()))
+        return lp, lmass, nsp
+
+    def teacher_force(self, plen: int, prefill: bool, nospeech_pos: Optional[int] = None) -> None:
+        """Run the teacher-forced positions 0..plen-2 of the decode just begun: one batched prefill pass when `prefill`, else
+        decoder steps.  nospeech_pos (scores on): the prefill stops before that position, and the positions from it on run as steps,
+        because the prefill has no LM head and the no-speech probability is read from the step that consumes it."""
+        split = plen - 1 if nospeech_pos is None else min(plen - 1, nospeech_pos)
+        if prefill and split >= 1:
+            self.decode_prefill(split)
+            self.decode_run(plen - 1 - split)
+            self.stats["sot_split_steps"] += plen - 1 - split
+        else:
+            self.decode_run(plen - 1)
+
     def graph_stats(self) -> Dict[str, float]:
         """The engine's step-graph cache: graphs captured, seconds spent capturing them, graphs cached now, graphs evicted."""
         out = (C.c_int64 * 4)()
@@ -411,18 +444,18 @@ class WhisperEngine:
         return self.buffer("logits", torch.float32, (self.max_audios * self.max_beams, vp))[: self._Q, : self.dims.vocab]
 
     def greedy(self, prompts: np.ndarray, A: int, opts: DecodeOptions, max_new_tokens: int, poll_every: int = 32,
-               prefill: bool = False, key_start: Optional[Sequence[int]] = None):
+               prefill: bool = False, key_start: Optional[Sequence[int]] = None, nospeech: Optional[Sequence[int]] = None):
         """Greedy decode of A audios (their cross K/V must be resident from encode()).  Returns generated ids per
         audio (prompt stripped, cut at and excluding EOS) and the raw token matrix.  prefill: run the teacher-forced
-        positions as one batched prefill pass instead of step by step.  key_start: see decode_begin."""
+        positions as one batched prefill pass instead of step by step.  key_start: see decode_begin.  nospeech = (position,
+        token): scores on (decode_scores_enable, teacher_force); read them with decode_scores afterwards."""
         plen = prompts.shape[1]
         Tmax = self.dims.max_target_positions
         max_new = max(0, min(max_new_tokens, Tmax - plen))
         self.decode_begin(prompts, A, 1, opts, key_start=key_start)
-        if prefill and plen > 1:  # teacher-forced prompt positions 0..plen-2
-            self.decode_prefill(plen - 1)
-        else:
-            self.decode_run(plen - 1)
+        if nospeech is not None:
+            self.decode_scores_enable(*nospeech)
+        self.teacher_force(plen, prefill, None if nospeech is None else nospeech[0])
         done = 0
         toks = fin = None
         while done < max_new:

@@ -15,8 +15,10 @@ What is covered (everything the reference's ASRPipeline / LocalWhisperBackend re
   * condition_on_prev_tokens: [<|startofprev|> or the prompt (prompt_condition_type="all-segments"), last 223 tokens of the
     row's text] + init tokens, rows left-padded to the longest and the pads masked by a per-row key start in decoder
     self-attention (:1853-1915); the conditioning positions run as one batched prefill pass
-Not covered (long-form only): temperature fallback, logprob / compression-ratio thresholds, no-speech skipping -- sampling is not
-part of the engine.
+  * no-speech skipping at temperature 0 (no_speech_threshold with logprob_threshold, _need_fallback's should_skip): avg_logprob from
+    the processed log-probs the select kernel records, no_speech_prob from the raw logits of the step whose input is
+    <|startoftranscript|> (WhisperNoSpeechDetection), in short and long form, greedy and beam
+Not covered: temperature fallback and the compression-ratio threshold's fallback -- sampling is not part of the engine.
 """
 from __future__ import annotations
 
@@ -146,30 +148,73 @@ class WhisperGenerator:
 
     # --------------------------------------------------------------------------------------------------------
     def _decode(self, prompts: np.ndarray, A: int, opts: DecodeOptions, max_new: int, num_beams: int, prefill: bool = False,
-                key_start=None):
+                key_start=None, n_init: Optional[int] = None):
         """-> (list of generated id arrays cut before EOS, n_steps HF would have run, eos_seen per row).  prefill: the
         teacher-forced positions run as one batched prefill pass (a prompt), not step by step.  key_start [A]: left-padded
-        prompts, the positions below it are masked (engine.decode_begin)."""
+        prompts, the positions below it are masked (engine.decode_begin).  n_init (no-speech skipping): the decode runs with scores,
+        and self._window_scores = (avg_logprob [A], no_speech_prob [A]) of the window afterwards (_nospeech_stats)."""
         self._beam_indices = None
+        self._window_scores = None
+        plen = prompts.shape[1]
         kw = {"prefill": True} if prefill else {}
         if key_start is not None:
             kw["key_start"] = key_start
+        if n_init is not None:  # the no-speech probability is read where <|startoftranscript|> is the input
+            kw["nospeech"] = (plen - n_init, self.st.no_timestamps_token_id - 1)
         if num_beams > 1:
             from .beam import beam_search
 
-            if opts.record_alignment:  # token timestamps need to know which slot produced each token of the winner
-                gen, steps, eos_seen, self._beam_indices = beam_search(self.eng, prompts, A, num_beams, opts, max_new, return_beam_indices=True, **kw)
-                return gen, steps, eos_seen
-            return beam_search(self.eng, prompts, A, num_beams, opts, max_new, **kw)
+            want_bidx = opts.record_alignment or n_init is not None  # which slot produced each token of the winner
+            res = beam_search(self.eng, prompts, A, num_beams, opts, max_new, return_beam_indices=want_bidx, **kw)
+            gen, steps, eos_seen = res[:3]
+            if want_bidx:
+                self._beam_indices = res[3]
+            if n_init is not None:
+                seqs = [self._hf_row(np.concatenate([g, [opts.eos_token]]) if e else g, opts) for g, e in zip(gen, eos_seen)]
+                self._window_scores = self._nospeech_stats(seqs, plen, n_init, num_beams, tlp=res[4])
+            return gen, steps, eos_seen
         gen, toks, done = self.eng.greedy(prompts, A, opts, max_new, **kw)
-        plen = prompts.shape[1]
         first_eos = []
         for a in range(A):
             row = toks[a, plen:plen + done]
             w = np.where(row == opts.eos_token)[0]
             first_eos.append(int(w[0]) + 1 if len(w) else done)
         n_steps = min(done, max(first_eos)) if A else 0
+        if n_init is not None:
+            seqs = [self._hf_row(toks[a, plen:plen + n_steps], opts) for a in range(A)]
+            self._window_scores = self._nospeech_stats(seqs, plen, n_init, 1)
         return gen, n_steps, [fe <= done and (toks[a, plen:plen + done] == opts.eos_token).any() for a, fe in enumerate(first_eos)]
+
+    @staticmethod
+    def _hf_row(row: np.ndarray, opts: DecodeOptions) -> np.ndarray:
+        """The sequence transformers scores (generate_with_fallback): trailing pads dropped, one kept when pad is EOS."""
+        row = np.asarray(row, dtype=np.int64)
+        if len(row) and row[-1] == opts.pad_token:
+            n = int((row == opts.pad_token).sum()) - (1 if opts.pad_token == opts.eos_token else 0)
+            if n:
+                row = row[:-n]
+        return row
+
+    def _nospeech_stats(self, seqs: List[np.ndarray], plen: int, n_init: int, G: int, tlp: Optional[np.ndarray] = None):
+        """avg_logprob and no_speech_prob per row (_retrieve_avg_logprobs, WhisperNoSpeechDetection).  Greedy: the mean of the
+        processed log-probs of the row's tokens.  Beam: along the winner's `beam_indices`, raw log-prob minus the slot's lmass at
+        that step.  no_speech_prob is read at slot a * G, except when n_init == 1 under beam search: transformers then reads row a
+        of its beam-expanded first-step scores, which is slot a."""
+        lp, lmass, nsp = self.eng.decode_scores()
+        A = len(seqs)
+        avg = np.zeros(A, dtype=np.float64)
+        for a, seq in enumerate(seqs):
+            n = len(seq)
+            if n == 0:
+                continue
+            if G > 1:
+                slots = self._beam_indices[a, :n]
+                vals = tlp[a, :n].astype(np.float64) - lmass[slots, plen + np.arange(n)]
+            else:
+                vals = lp[a, plen:plen + n].astype(np.float64)
+            avg[a] = vals.sum() / n
+        ns = nsp[np.arange(A)] if (G > 1 and n_init == 1) else nsp[np.arange(A) * G]
+        return avg, ns.astype(np.float64)
 
     def _token_timestamps(self, A: int, plen: int, n_steps: int, num_frames: np.ndarray) -> List[np.ndarray]:
         """HF layout: zeros for the prompt, one time per generated position, last one duplicated (:375-379)."""
@@ -281,7 +326,8 @@ class WhisperGenerator:
                  return_timestamps: bool = False, return_token_timestamps: bool = False, language=None, task=None,
                  num_beams: int = 1, max_new_tokens: Optional[int] = None, extra_suppress: Sequence[int] = (),
                  encoded: bool = False, prompt_ids=None, prompt_condition_type: Optional[str] = None,
-                 max_frames: Optional[np.ndarray] = None, condition_on_prev_tokens: bool = False):
+                 max_frames: Optional[np.ndarray] = None, condition_on_prev_tokens: bool = False,
+                 no_speech_threshold: Optional[float] = None, logprob_threshold: Optional[float] = None):
         """Returns a dict with "sequences" (list of int arrays: generated ids, prompt and EOS stripped), optionally
         "token_timestamps" (list of float arrays aligned with sequences) and "segments".
 
@@ -295,7 +341,16 @@ class WhisperGenerator:
         transformers' generate does (generation_whisper.py _prepare_decoder_input_ids).
         condition_on_prev_tokens: from the second window on, the decoder input of every row is [<|startofprev|> (or the prompt),
         last 223 tokens of its text so far] + init tokens, the rows left-padded to the longest; the pads are masked by a key start
-        per row.  The conditioning positions run through the decoder in one batched prefill pass."""
+        per row.  The conditioning positions run through the decoder in one batched prefill pass.
+        no_speech_threshold with logprob_threshold (both or neither): a window of a row is skipped -- no tokens, no segment, `seek`
+        moves by the window's frame count, the row's history is unchanged -- when its avg_logprob < logprob_threshold and its
+        no_speech_prob > no_speech_threshold, as transformers decides it at one temperature (_need_fallback).  The decode then runs
+        with scores (engine.decode_scores_enable); with a prompt or history the prefill stops before <|startoftranscript|>.
+        self.window_stats["skipped"] counts skipped windows over all rows, and self.window_log holds per window the (avg_logprob, no_speech_prob,
+        skipped) of each of its rows."""
+        if (no_speech_threshold is None) != (logprob_threshold is None):
+            raise ValueError("no_speech_threshold and logprob_threshold go together: set both or neither")
+        nospeech = no_speech_threshold is not None
         eng, st = self.eng, self.st
         if prompt_condition_type not in (None, "first-segment", "all-segments"):
             raise ValueError(f"`prompt_condition_type={prompt_condition_type} does not exist. Make sure to set `prompt_condition_type` "
@@ -354,7 +409,8 @@ class WhisperGenerator:
             segments = [[{"tokens": p0.astype(np.int64)}] for _ in range(B)]
             n_hidden = 1
         tb = self.timestamp_begin
-        self.window_stats = {"windows": 0, "conditioned": 0, "left_padded": 0, "history_cut": 0}
+        self.window_stats = {"windows": 0, "conditioned": 0, "left_padded": 0, "history_cut": 0, "skipped": 0}
+        self.window_log = []
 
         seek = np.zeros(B, dtype=np.int64)
         first = True
@@ -403,11 +459,22 @@ class WhisperGenerator:
             kw = {"prefill": True} if plen > n_init else {}
             if key_start is not None:
                 kw["key_start"] = key_start
+            if nospeech:
+                kw["n_init"] = n_init
             gen, n_steps, _ = self._decode(prompts, A, opts, max_new, num_beams, **kw)
+            skip = np.zeros(A, dtype=bool)
+            if nospeech:
+                avg_lp, ns_prob = self._window_scores
+                skip = (avg_lp < logprob_threshold) & (ns_prob > no_speech_threshold)
+                self.window_stats["skipped"] += int(skip.sum())
+                self.window_log.append([(float(avg_lp[j]), float(ns_prob[j]), bool(skip[j])) for j in range(A)])
             tts = None
             if return_token_timestamps:
                 tts = self._token_timestamps(A, plen, n_steps, (num_frames - seek)[rows])
             for j, i in enumerate(rows):
+                if skip[j]:  # (generate_with_fallback's should_skip)
+                    seek[i] += seek_num_frames[i]
+                    continue
                 seq = np.asarray(gen[j], dtype=np.int64)
                 time_offset = float(seek[i]) * self.time_precision / 2.0  # (float64, as transformers computes it off the MPS device)
                 if len(seq) == 0:  # (HF runs _retrieve_segment in every mode: timestamp ids are not masked without timestamps)

@@ -9,7 +9,9 @@ return_timestamps=None|True|"word", return_language=..., batch_size=..., generat
 Without chunk_length_s, an input longer than the window is transcribed with Whisper's sequential long-form algorithm (as
 transformers' pipeline does): inputs are grouped batch_size at a time, a group whose longest item fits the window takes the
 one-window path, any other group the long-form seek loop of WhisperGenerator.generate (timestamps on; generate_kwargs
-condition_on_prev_tokens / prompt_condition_type as in transformers).
+condition_on_prev_tokens / prompt_condition_type as in transformers).  generate_kwargs no_speech_threshold with logprob_threshold
+skip the windows transformers skips at one temperature, in every mode (the item's text is "" in short form);
+compression_ratio_threshold is accepted next to them and has no effect, as in transformers at one temperature.
 
 Everything numeric below the call -- log-mel, encoder, decoder, logits rules, token selection, DTW -- runs in the CUDA
 engine through the C-ABI.  What stays on the host is what the reference keeps on the host too: the window schedule of
@@ -182,9 +184,14 @@ class ASRPipeline:
         if isinstance(temperature, (list, tuple)) or (temperature is not None and temperature > 0.0):
             raise NotImplementedError(f"temperature={temperature!r}: temperature fallback samples, and sampling is not part of the engine "
                                       "(greedy / beam only)")
-        for name in ("logprob_threshold", "compression_ratio_threshold", "no_speech_threshold"):
-            if generate_kwargs.get(name) is not None:
-                raise NotImplementedError(f"{name} is not implemented: the engine has no temperature fallback or no-speech skipping")
+        # no-speech skipping needs both thresholds; at one temperature compression_ratio_threshold only marks a fallback that
+        # never runs, so next to them it is accepted and has no effect (as in transformers)
+        no_speech = generate_kwargs.get("no_speech_threshold") is not None and generate_kwargs.get("logprob_threshold") is not None
+        if not no_speech:
+            for name in ("logprob_threshold", "compression_ratio_threshold", "no_speech_threshold"):
+                if generate_kwargs.get(name) is not None:
+                    raise NotImplementedError(f"{name} is not implemented: the engine has no temperature fallback, and no-speech "
+                                              "skipping needs both no_speech_threshold and logprob_threshold")
         condition = bool(generate_kwargs.get("condition_on_prev_tokens") or False)
         num_beams = int(generate_kwargs.get("num_beams", 1) or 1)
         if num_beams > self.max_beams:
@@ -230,7 +237,8 @@ class ASRPipeline:
                 return_token_timestamps=(return_timestamps == "word"), language=generate_kwargs.get("language"),
                 task=generate_kwargs.get("task"), num_beams=num_beams, max_new_tokens=generate_kwargs.get("max_new_tokens"),
                 prompt_ids=generate_kwargs.get("prompt_ids"), prompt_condition_type=generate_kwargs.get("prompt_condition_type"),
-                condition_on_prev_tokens=condition, **long_kw)
+                condition_on_prev_tokens=condition, no_speech_threshold=generate_kwargs.get("no_speech_threshold") if no_speech else None,
+                logprob_threshold=generate_kwargs.get("logprob_threshold") if no_speech else None, **long_kw)
             for j, g in enumerate(group):
                 o: Dict[str, Any] = {"tokens": np.asarray(out["sequences"][j], dtype=np.int64)[None, :]}
                 if return_timestamps == "word":
